@@ -341,6 +341,15 @@ class Accl:
         return self._a.alltoall(_impl(sendbuf), _impl(recvbuf), count, comm_id, from_fpga, to_fpga,
                                 self._cd(compress_dtype), run_async)
 
+    def alltoallv(self, sendbuf, recvbuf, counts, comm_id=GLOBAL_COMM, from_fpga=False, to_fpga=False, run_async=False):
+        """Uneven all-to-all.  `counts`: int64 buffer of at least 2P elements that the engine reads (on the CUDA
+        backend it must be device resident): counts[q] elements go to rank q, counts[P + p] come from rank p, packed
+        in rank order in both buffers.  The buffers' lengths are the capacities.  Counts that disagree anywhere in
+        the communicator (a send count unlike its receiver's count, a negative count, more than a buffer holds)
+        fail the call with DMA_SIZE_ERROR on every rank, and no receive buffer is written."""
+        self._stream()
+        return self._a.alltoallv(_impl(sendbuf), _impl(recvbuf), _impl(counts), comm_id, from_fpga, to_fpga, run_async)
+
     def barrier(self, comm_id=GLOBAL_COMM):
         self._stream()
         return self._a.barrier(comm_id)

@@ -7,7 +7,7 @@ them on a H100 node:
 
 * `init_from_env`        one rank per process (torchrun): pick the backend, build the world
 * `TensorGroup`          torch-tensor front end: all_reduce / all_gather / reduce_scatter /
-                         broadcast / all_to_all / send / recv on CUDA tensors (zero-copy when the
+                         broadcast / all_to_all (even or uneven) / send / recv on CUDA tensors (zero-copy when the
                          tensor already lives in the symmetric heap, staged otherwise)
 * `GradBucket`           DP / ZeRO gradient bucket living in the heap: fill, then one all-reduce
                          (or reduce_scatter + all_gather) per bucket, stream ordered
@@ -195,6 +195,29 @@ class TensorGroup:
     def all_to_all_single(self, out: torch.Tensor, inp: torch.Tensor):
         n = inp.numel() // self.world
         return self._run(lambda s, d: self.accl.alltoall(s, d, n, self.comm_id, self._res, self._res, run_async=self._async), inp, out, n * self.world, n * self.world)
+
+    def all_to_all_v(self, out: torch.Tensor, inp: torch.Tensor, send_counts: torch.Tensor, recv_counts: torch.Tensor):
+        """Uneven all-to-all in elements: send_counts[q] elements of `inp` go to rank q and recv_counts[p] elements
+        from rank p land in `out`, both packed in rank order.  The counts are int64 tensors of `world` elements (on
+        the GPU for the CUDA backend); they are packed with device copies and read by the engine, so nothing waits
+        for the host.  Capacities are inp.numel() and out.numel().  The elements of `out` past the received blocks
+        keep their values when `out` lives in the heap; a staged `out` gets the staging buffer's there (undefined)."""
+        P = self.world
+        cb = self._scratch.get(("counts", P))
+        if cb is None:
+            cb = self._scratch[("counts", P)] = self.accl.create_buffer(2 * P, torch.int64)
+        ct = self._t(cb)
+        ct[:P].copy_(send_counts.reshape(-1))
+        ct[P:2 * P].copy_(recv_counts.reshape(-1))
+
+        def fn(s, d):
+            # a staging buffer may be longer than the tensor: the capacities are the tensors' own lengths
+            s = s if s.length == inp.numel() else s.slice(0, inp.numel())
+            d = d if d.length == out.numel() else d.slice(0, out.numel())
+            return self.accl.alltoallv(s, d, cb, self.comm_id, self._res, self._res, run_async=self._async)
+        # a rank may send or receive nothing: stage through one element, pass a capacity of zero
+        src, dst = (inp if inp.numel() else inp.new_empty(1)), (out if out.numel() else out.new_empty(1))
+        return self._run(fn, src, dst, inp.numel(), out.numel())
 
     def send(self, t: torch.Tensor, dst, tag=0):
         sb, staged = self._buffer_of(t, "s")

@@ -10,6 +10,7 @@ extension are available (tensors must then be CUDA tensors; calls are stream ord
 complete immediately, like NCCL's), otherwise the CPU emulator over loopback TCP (calls are blocking).
 SURVEY 7.2 step 9 ("optional ProcessGroup shim for drop-in comparison").
 """
+import math
 import os
 
 import torch
@@ -174,9 +175,19 @@ class AcclProcessGroup(dist.ProcessGroup):
 
     def alltoall_base(self, output_buffer, input_buffer, output_split_sizes, input_split_sizes, opts=AllToAllOptions()):
         self._join()
-        if output_split_sizes or input_split_sizes:
-            raise NotImplementedError("accl backend: all_to_all_single with uneven splits")
-        self.group.all_to_all_single(output_buffer, input_buffer.contiguous())
+        if not output_split_sizes and not input_split_sizes:
+            self.group.all_to_all_single(output_buffer, input_buffer.contiguous())
+            return _done(output_buffer)
+        # uneven: splits are dim-0 rows (an empty list means even splits); the engine takes element counts
+        P = self._world
+        row = math.prod(input_buffer.shape[1:])   # from the trailing dimensions: a rank may send zero rows
+        if math.prod(output_buffer.shape[1:]) != row:
+            raise ValueError("accl backend: all_to_all_single with input and output rows of different sizes")
+        in_splits = list(input_split_sizes) or [input_buffer.shape[0] // P] * P
+        out_splits = list(output_split_sizes) or [output_buffer.shape[0] // P] * P
+        dev = input_buffer.device if self.accl.is_cuda else "cpu"
+        counts = torch.tensor(in_splits + out_splits, dtype=torch.int64, device=dev) * row
+        self.group.all_to_all_v(output_buffer, input_buffer.contiguous(), counts[:P], counts[P:])
         return _done(output_buffer)
 
     def alltoall(self, output_tensor_list, input_tensor_list, opts=AllToAllOptions()):

@@ -6,6 +6,7 @@ emulator and on H100, and is covered by tests/test_parallel.py.
 * `ColumnParallelLinear`     Megatron column-parallel linear (local GEMM; optional all_gather of the output)
 * `pipeline_send` / `pipeline_recv`   tagged activation hand-off between pipeline stages
 * `moe_dispatch` / `moe_combine`      expert-parallel token exchange (all_to_all, equal capacity per expert rank)
+* `moe_dispatch_v` / `moe_combine_v`  dropless token exchange (alltoallv: routed row counts stay on the device)
 * `ulysses_seq_to_head` / `ulysses_head_to_seq`   DeepSpeed-Ulysses re-sharding sequence <-> heads (all_to_all)
 """
 import torch
@@ -92,6 +93,31 @@ def moe_dispatch(group: TensorGroup, tokens_by_dest: torch.Tensor):
 def moe_combine(group: TensorGroup, expert_out_by_src: torch.Tensor):
     """Inverse of `moe_dispatch`: send every processed block back to the rank it came from."""
     return moe_dispatch(group, expert_out_by_src)
+
+
+def moe_dispatch_v(group: TensorGroup, tokens: torch.Tensor, send_counts: torch.Tensor, capacity: int):
+    """Dropless dispatch.  tokens: [N, hidden], rows grouped by destination rank in rank order; send_counts: int64
+    rows per destination (on the device for the CUDA backend).  The row counts are exchanged first (one int64 per
+    peer), then the rows move with alltoallv into a [capacity, hidden] buffer; no step waits for the host.
+    Returns (recv_tokens, recv_counts): recv_counts[p] rows from rank p, packed in rank order."""
+    hidden = tokens.shape[1]
+    send_counts = send_counts.to(torch.int64).contiguous()
+    recv_counts = torch.empty_like(send_counts)
+    group.all_to_all_single(recv_counts, send_counts)
+    recv = torch.empty(capacity, hidden, dtype=tokens.dtype, device=tokens.device)
+    group.all_to_all_v(recv.view(-1), tokens.contiguous().view(-1), send_counts * hidden, recv_counts * hidden)
+    return recv, recv_counts
+
+
+def moe_combine_v(group: TensorGroup, expert_out: torch.Tensor, recv_counts: torch.Tensor, send_counts: torch.Tensor,
+                  num_tokens: int):
+    """Inverse of `moe_dispatch_v`: the rows of `expert_out` ([capacity, hidden], recv_counts[p] rows from rank p)
+    go back to the ranks they came from.  Returns [num_tokens, hidden] in the original dispatch order."""
+    hidden = expert_out.shape[1]
+    out = torch.empty(num_tokens, hidden, dtype=expert_out.dtype, device=expert_out.device)
+    group.all_to_all_v(out.view(-1), expert_out.contiguous().view(-1), recv_counts.to(torch.int64) * hidden,
+                       send_counts.to(torch.int64) * hidden)
+    return out
 
 
 def ulysses_seq_to_head(group: TensorGroup, x: torch.Tensor):

@@ -99,7 +99,7 @@ PYBIND11_MODULE(_C, m) {
       .value("scatter", operation::scatter).value("gather", operation::gather).value("reduce", operation::reduce)
       .value("allgather", operation::allgather).value("allreduce", operation::allreduce)
       .value("reduce_scatter", operation::reduce_scatter).value("barrier", operation::barrier)
-      .value("alltoall", operation::alltoall).value("nop", operation::nop);
+      .value("alltoall", operation::alltoall).value("alltoallv", operation::alltoallv).value("nop", operation::nop);
   py::enum_<bufferKind>(m, "BufferKind")
       .value("device", bufferKind::device).value("host_only", bufferKind::host_only).value("p2p", bufferKind::p2p);
   py::enum_<deviceType>(m, "DeviceType").value("emulator", deviceType::emulator).value("cuda", deviceType::cuda);
@@ -273,6 +273,10 @@ PYBIND11_MODULE(_C, m) {
       }, py::arg("sendbuf"), py::arg("recvbuf"), py::arg("count"), py::arg("comm_id") = GLOBAL_COMM,
            py::arg("from_fpga") = false, py::arg("to_fpga") = false, py::arg("compress_dtype") = dataType::none,
            py::arg("run_async") = false, gil_release())
+      .def("alltoallv", [](ACCL &a, BaseBuffer &s, BaseBuffer &r, BaseBuffer &counts, unsigned comm, bool from_fpga, bool to_fpga,
+                           bool async_) { return wrap(a, a.alltoallv(s, r, counts, comm, from_fpga, to_fpga, async_)); },
+           py::arg("sendbuf"), py::arg("recvbuf"), py::arg("counts"), py::arg("comm_id") = GLOBAL_COMM,
+           py::arg("from_fpga") = false, py::arg("to_fpga") = false, py::arg("run_async") = false, gil_release())
       .def("barrier", [](ACCL &a, unsigned comm) { a.free_request(a.barrier(comm)); }, py::arg("comm_id") = GLOBAL_COMM, gil_release())
       .def("create_communicator", &ACCL::create_communicator, py::arg("ranks"), py::arg("local_rank"))
       .def("get_comm_group", &ACCL::get_comm_group)

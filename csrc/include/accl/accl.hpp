@@ -137,6 +137,14 @@ public:
                         communicatorId comm_id = GLOBAL_COMM, bool from_fpga = false, bool to_fpga = false,
                         dataType compress_dtype = dataType::none, bool run_async = false,
                         std::vector<ACCLRequest *> waitfor = {});
+  // Uneven all-to-all.  `counts` (int64, at least 2P elements, P = communicator size) is read by the engine:
+  // counts[q] = elements this rank sends to rank q, counts[P + p] = elements it receives from rank p.  Blocks are
+  // packed in rank order (exclusive prefix sums of the counts) in both buffers; their lengths are the capacities.
+  // An inconsistent count matrix anywhere in the communicator fails the call with DMA_SIZE_ERROR on every rank
+  // without writing any receive buffer.
+  ACCLRequest *alltoallv(BaseBuffer &sendbuf, BaseBuffer &recvbuf, BaseBuffer &counts,
+                         communicatorId comm_id = GLOBAL_COMM, bool from_fpga = false, bool to_fpga = false,
+                         bool run_async = false, std::vector<ACCLRequest *> waitfor = {});
   ACCLRequest *barrier(communicatorId comm_id = GLOBAL_COMM, std::vector<ACCLRequest *> waitfor = {});
 
   // ---- requests
@@ -214,6 +222,9 @@ private:
 
   std::unique_ptr<CCLO> cclo;
   arithConfigMap arith_config;
+  // one extra exchange-memory entry, outside `arith_config`: the element width of 1-byte payloads (int8, fp8) that
+  // alltoallv moves as bytes; every other call on such buffers is still refused by the lookup in prepare_call
+  ArithConfig byte_move_config_{dataType::int8, dataType::int8, 0, false};
   std::vector<Communicator> communicators;
   std::vector<std::shared_ptr<BufferStorage>> eager_rx_buffers;
   std::vector<std::shared_ptr<BufferStorage>> spare_buffers;

@@ -24,6 +24,9 @@ namespace accl {
 // the reference's stream ABI (driver/hls/accl_hls.h:134-198):
 // scenario, count, comm, root_src_dst, function, tag, arithcfg,
 // compression_flags, stream_flags|host_flags<<8, addr a/b/c as lo/hi pairs.
+//
+// alltoallv reuses two words: addr0 = send buffer, addr1 = int64 counts (2P), addr2 = receive buffer;
+// `count` = receive capacity and `root_src_dst` (unused: no root) = send capacity, both in elements.
 struct alignas(64) CallDesc {
   uint32_t scenario;
   uint32_t count;

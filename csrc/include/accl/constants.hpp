@@ -44,6 +44,7 @@ enum class operation : uint32_t {
   reduce_scatter = 11,
   barrier = 12,
   alltoall = 13,
+  alltoallv = 14, // uneven all-to-all, per-peer counts read from device memory (beyond the reference)
   nop = 255
 };
 const char *operation_name(operation op);

@@ -95,6 +95,14 @@ ACCL_HD void plan_call(const uint32_t *exch, const PlanCfg &cfg, WorkItem &w) {
     w.n_ctas = 1;
     return;
   }
+  if (op == operation::alltoallv) {
+    // the block sizes live in device memory and `count` is this rank's receive capacity, which differs between
+    // ranks: every channel decision here must come from configuration alone, or the ranks' grids (and with them
+    // the per-channel meetings) would disagree.  Always the rendezvous push between user buffers.
+    w.algo = ALGO_P2P;
+    w.n_ctas = cap;
+    return;
+  }
   uint64_t moved = ubytes; // payload a rank moves, for sizing
   if (op == operation::allgather || op == operation::reduce_scatter || op == operation::alltoall ||
       op == operation::scatter || op == operation::gather)
@@ -209,9 +217,10 @@ ACCL_HD uint32_t build_work_item_hd(const uint32_t *exch, const PlanCfg &cfg, ui
   const bool rooted = op == operation::send || op == operation::recv || op == operation::bcast ||
                       op == operation::scatter || op == operation::gather || op == operation::reduce;
   if (rooted && d.root_src_dst >= w.comm_size) return CONFIG_SWITCH_ERROR;
-  // a communicator of one: every collective degenerates to a local copy
+  // a communicator of one: every collective degenerates to a local copy (alltoallv excepted: its size is in device
+  // memory, its body validates and copies it)
   if (w.comm_size == 1 && op != operation::copy && op != operation::combine && op != operation::nop &&
-      op != operation::config) {
+      op != operation::config && op != operation::alltoallv) {
     if (op == operation::barrier || op == operation::bcast) w.desc.scenario = static_cast<uint32_t>(operation::nop);
     else if (op == operation::send || op == operation::recv) return CONFIG_SWITCH_ERROR; // no loop-back slots to self
     else w.desc.scenario = static_cast<uint32_t>(operation::copy);

@@ -175,6 +175,7 @@ private:
   uint32_t fw_allreduce(EmuCall &c);
   uint32_t fw_barrier(EmuCall &c);
   uint32_t fw_alltoall(EmuCall &c);
+  uint32_t fw_alltoallv(EmuCall &c);
   void soft_reset();
 
   struct Ctx; // decoded call context (engine.cpp)
@@ -242,7 +243,8 @@ private:
   // rendezvous mailboxes (guarded by q_m_ so arrivals wake the control loop)
   // kind: what posted the note (1 = point to point, 0x100 | opcode = that collective) — a send must never take
   // the address a collective announced with TAG_ANY, and vice versa
-  struct AddrNote { uint32_t comm_sig, src, tag, count; uint64_t vaddr; uint32_t kind; };
+  // payload: what an alltoallv announces with its buffer (its counts and capacities)
+  struct AddrNote { uint32_t comm_sig, src, tag, count; uint64_t vaddr; uint32_t kind; std::vector<uint8_t> payload; };
   struct DoneNote { uint32_t comm_sig, src, tag; bool barrier; uint32_t kind; };
   std::list<AddrNote> addr_notes_;
   std::list<DoneNote> done_notes_;

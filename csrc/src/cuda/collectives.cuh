@@ -577,6 +577,100 @@ __device__ __noinline__ void rvb_move(const Ctx &c, Pattern pat, const uint64_t 
   }
 }
 
+// ---------------------------------------------------------------- alltoallv
+// The counts of an alltoallv live in device memory (int64: P send counts, then P receive counts, in elements).  At
+// the entry meeting a rank publishes the heap offset of its counts in the off0 slot (the push bodies never read a
+// peer's source offset) and its receive buffer in off2.  A rank whose counts fail the checks only it can make (a
+// negative count, more than its buffers hold) publishes A2AV_REJECT instead, so that every rank fails the call.
+// INVALID_OFF already means "this peer timed out".
+constexpr uint64_t A2AV_REJECT = ~0ull - 1;
+
+// What this rank publishes in off0 (every calling thread computes the same value).  Relaxed .sys loads: the engine
+// kernel outlives the host writes to a counts buffer, so nothing may come from a stale L1 line.
+__device__ __noinline__ uint64_t a2av_entry_off(const char *heap, const WorkItem &it) {
+  const uint64_t *cnt = reinterpret_cast<const uint64_t *>(heap + it.desc.addr1());
+  const uint32_t P = it.comm_size;
+  const int64_t scap = it.desc.root_src_dst, rcap = it.desc.count;
+  int64_t s = 0, r = 0;
+  bool ok = true;
+  for (uint32_t q = 0; q < P; ++q) {
+    const int64_t a = static_cast<int64_t>(ld_relaxed_sys(cnt + q)), b = static_cast<int64_t>(ld_relaxed_sys(cnt + P + q));
+    ok = ok && a >= 0 && a <= scap && b >= 0 && b <= rcap; // bounded first: the sums below cannot overflow
+    s += ok ? a : 0;
+    r += ok ? b : 0;
+  }
+  return ok && s <= scap && r <= rcap ? it.desc.addr1() : A2AV_REJECT;
+}
+
+__device__ __forceinline__ int64_t a2av_count(const Ctx &c, const uint64_t *s_off0, uint32_t p, uint32_t i) {
+  return static_cast<int64_t>(ld_relaxed_sys(reinterpret_cast<const uint64_t *>(c.heap(c.g(p)) + s_off0[p]) + i));
+}
+
+// `bytes` from src to dst split over (cta, nctas) on the widest path the two addresses allow: 16-byte vectors when
+// they are congruent mod 16 (head and tail peeled), 4-byte words when congruent mod 4, else bytes.  Arbitrary
+// element counts put the blocks at arbitrary byte offsets, where copy_simple would fall back to single bytes.
+__device__ __forceinline__ void copy_congruent(char *dst, const char *src, size_t bytes, int cta, int nctas) {
+  const uintptr_t d = reinterpret_cast<uintptr_t>(dst), x = d ^ reinterpret_cast<uintptr_t>(src);
+  const size_t g = (x & 15) == 0 ? 16 : ((x & 3) == 0 ? 4 : 1);
+  size_t head = (g - (d & (g - 1))) & (g - 1);
+  if (head > bytes) head = bytes;
+  const size_t body = (bytes - head) / g * g;
+  const size_t stride = static_cast<size_t>(nctas) * blockDim.x;
+  const size_t tid = static_cast<size_t>(cta) * blockDim.x + threadIdx.x;
+  for (size_t i = tid; i < head; i += stride) dst[i] = *reinterpret_cast<const volatile char *>(src + i);
+  for (size_t i = head + body + tid; i < bytes; i += stride) dst[i] = *reinterpret_cast<const volatile char *>(src + i);
+  if (g == 4) {
+    uint32_t *dw = reinterpret_cast<uint32_t *>(dst + head);
+    const volatile uint32_t *sw = reinterpret_cast<const volatile uint32_t *>(src + head);
+    for (size_t i = tid; i < body / 4; i += stride) dw[i] = sw[i];
+  } else {
+    copy_simple(dst + head, src + head, body, cta, nctas); // g == 16: the vector path; g == 1: bytes
+  }
+}
+
+// Data phase of alltoallv.  Every CTA checks the whole count matrix from the peers' counts buffers (at most 2 x 16 x
+// 16 loads), so all ranks reach the same verdict; the peers wrote their counts with stream-ordered work before their
+// kernels started, and nobody leaves the exit meeting before everybody has read them.  Then each CTA pushes its
+// share of every block, starting at a different destination.
+__device__ __noinline__ void rvb_alltoallv(const Ctx &c, const uint64_t *s_off0, const uint64_t *s_off2) {
+  __shared__ uint64_t s_len[ACCL_MAX_RANKS];
+  __shared__ uint32_t s_bad;
+  const WorkItem &it = c.it;
+  const uint32_t P = c.P(), me = c.r(), t = threadIdx.x;
+  const size_t es = esize(it.udtype);
+  __syncthreads();
+  if (t == 0) s_bad = 0;
+  __syncthreads();
+  if (t < P && (s_off0[t] == A2AV_REJECT || s_off0[t] > c.w.heap_bytes - 16ull * P)) s_bad = 1;
+  __syncthreads();
+  if (!s_bad)
+    for (uint32_t i = t; i < P * P; i += blockDim.x) {
+      const uint32_t p = i / P, q = i % P; // p's send count to q against q's receive count from p
+      if (a2av_count(c, s_off0, p, q) != a2av_count(c, s_off0, q, P + p)) s_bad = 1;
+    }
+  __syncthreads();
+  if (s_bad) {
+    if (t == 0) atomicOr(c.err, DMA_SIZE_ERROR);
+    return;
+  }
+  if (t < P) {
+    // my block for q: at the prefix of my send counts in my source, after the blocks of q's lower senders in q's
+    // destination
+    const uint32_t q = t;
+    uint64_t so = 0, dof = 0;
+    for (uint32_t j = 0; j < q; ++j) so += a2av_count(c, s_off0, me, j);
+    for (uint32_t p = 0; p < me; ++p) dof += a2av_count(c, s_off0, q, P + p);
+    c.tab->src[q] = c.heap(c.w.rank) + it.desc.addr0() + so * es;
+    c.tab->dst[q] = c.heap(c.g(q)) + s_off2[q] + dof * es;
+    s_len[q] = a2av_count(c, s_off0, me, q) * es;
+  }
+  __syncthreads();
+  for (uint32_t k = 0; k < P; ++k) {
+    const uint32_t q = (me + k + static_cast<uint32_t>(c.cta)) % P; // all switch ports fed at once
+    copy_congruent(c.tab->dst[q], c.tab->src[q], s_len[q], c.cta, c.nctas);
+  }
+}
+
 // reduce to root.  Small: the root pulls (or lets the switch reduce) everything.  Large
 // (P >= 3): the P-1 other ranks each reduce one slice and store it into the root's buffer,
 // so the root's inbound link carries N bytes instead of (P-1) N.

@@ -146,6 +146,7 @@ struct Call { // one call in flight (running or parked) — lives in the control
   uint32_t step;   // current_step: where to resume
   uint32_t active;
   uint32_t err;
+  uint32_t body_err; // rendezvous collectives: error of the data phase, reported once the exit meeting is done
   uint32_t note_slot, note_seq; // rendezvous point-to-point
 };
 
@@ -162,7 +163,7 @@ __device__ __forceinline__ bool is_collective(uint32_t scenario) {
   const operation op = static_cast<operation>(scenario);
   return op == operation::bcast || op == operation::scatter || op == operation::gather || op == operation::reduce ||
          op == operation::allgather || op == operation::allreduce || op == operation::reduce_scatter ||
-         op == operation::barrier || op == operation::alltoall;
+         op == operation::barrier || op == operation::alltoall || op == operation::alltoallv;
 }
 
 // all threads; returns thread 0's value
@@ -442,7 +443,9 @@ __device__ uint32_t step_call(const EngCtx &e, Call &cl, uint32_t *s_err) {
   // exit meeting (parked until every member is done with my buffers)
   if (cl.step == 0) {
     const uint64_t my_dst = op == operation::bcast ? it.desc.addr0() : it.desc.addr2();
-    meet_post(e, cl, true, it.desc.addr0(), my_dst);
+    // alltoallv: the counts offset (or its local rejection, decided when the call was fetched) in the off0 slot
+    const uint64_t my_src = op == operation::alltoallv ? cl.off0[it.comm_rank] : it.desc.addr0();
+    meet_post(e, cl, true, my_src, my_dst);
     cl.step = 1;
   }
   if (cl.step == 1) {
@@ -455,10 +458,18 @@ __device__ uint32_t step_call(const EngCtx &e, Call &cl, uint32_t *s_err) {
   }
   if (cl.step == 3) {
     if (!move_finished(e, cl)) return SR_NOT_READY;
+    // a failed data phase (a rejected alltoallv) still meets its peers on the way out: a call retired before its exit
+    // meeting would leave that meeting to pair with the entry meeting of the next call on the bank
+    if (t == 0) {
+      cl.body_err = cl.err;
+      cl.err = 0;
+    }
     meet_post(e, cl, false, 0, 0);
     cl.step = 4;
   }
-  return meet_poll(e, cl, false) ? SR_DONE : SR_NOT_READY;
+  if (!meet_poll(e, cl, false)) return SR_NOT_READY;
+  if (t == 0) cl.err |= cl.body_err;
+  return SR_DONE;
 }
 
 // Ordering rules between calls in flight: collectives of one bank run one at a time in arrival order (their
@@ -520,6 +531,7 @@ __device__ void engine_control(const DevWorld &w, HostRing *hr, int nworkers) {
       __syncthreads();
       if (t == 0) {
         cl.err = 0;
+        cl.body_err = 0;
         if (!(cl.item.flags & WF_PLANNED)) {
           // device-issued descriptor: decode + plan here, from the device copy of exchange memory
           const CallDesc d = cl.item.desc;
@@ -536,6 +548,9 @@ __device__ void engine_control(const DevWorld &w, HostRing *hr, int nworkers) {
           s_host_fetched += 1;
         }
         cl.item.flags |= WF_ENGINE;
+        // alltoallv: this rank's own check of its counts, published at the entry meeting (collectives.cuh)
+        if (cl.item.desc.scenario == static_cast<uint32_t>(operation::alltoallv))
+          cl.off0[cl.item.comm_rank] = k::a2av_entry_off(w.window + static_cast<uint64_t>(w.rank) * w.heap_bytes, cl.item);
         cl.ticket1 = fetched + 1;
         cl.t_start = dev::globaltimer_ns();
         cl.step = 0;

@@ -29,8 +29,9 @@ __device__ __noinline__ void run_body(const Ctx &c, const uint64_t *off0, const 
   case operation::scatter:
   case operation::gather:
   case operation::alltoall: rvb_move(c, pattern_of(op), off0, off2, stepwise); break;
-  default:
-    if (threadIdx.x == 0) atomicOr(c.err, COLLECTIVE_NOT_IMPLEMENTED);
+  default: // (alltoallv here rather than as a case of its own: fewer registers saved around the calls above)
+    if (op == operation::alltoallv) rvb_alltoallv(c, off0, off2);
+    else if (threadIdx.x == 0) atomicOr(c.err, COLLECTIVE_NOT_IMPLEMENTED);
     break;
   }
 }
@@ -72,7 +73,8 @@ __device__ __noinline__ void run_work(const DevWorld &w, const WorkItem &it, int
     return;
   default: break;
   }
-  if (pat == PAT_NONE) {
+  const bool a2av = op == operation::alltoallv;
+  if (pat == PAT_NONE && !a2av) {
     if (threadIdx.x == 0) atomicOr(s_err, COLLECTIVE_NOT_IMPLEMENTED);
     return;
   }
@@ -81,8 +83,10 @@ __device__ __noinline__ void run_work(const DevWorld &w, const WorkItem &it, int
     return;
   }
   // rendezvous: entry meeting with the address exchange, data phase, exit meeting (the engine's step_call runs the
-  // same three steps).  Bcast keeps its buffer in addr0 on every rank; the others receive into addr2.
-  chan_sync(c, true, it.desc.addr0(), pat == PAT_BCAST ? it.desc.addr0() : it.desc.addr2(), s_off0, s_off2);
+  // same three steps).  Bcast keeps its buffer in addr0 on every rank; the others receive into addr2.  Alltoallv
+  // publishes its counts (or its rejection) in the off0 slot.
+  const uint64_t my_off0 = a2av ? a2av_entry_off(c.heap(w.rank), it) : it.desc.addr0();
+  chan_sync(c, true, my_off0, pat == PAT_BCAST ? it.desc.addr0() : it.desc.addr2(), s_off0, s_off2);
   if (*c.err == 0) run_body(c, s_off0, s_off2, true);
   chan_sync(c, false, 0, 0, nullptr, nullptr);
 }

@@ -340,7 +340,7 @@ void Engine::ingress_loop() {
     }
     case MsgType::RNDZVS_INIT: {
       std::lock_guard<std::mutex> g(q_m_);
-      addr_notes_.push_back(AddrNote{p.hdr.comm_sig, p.hdr.src, p.hdr.tag, p.hdr.count, p.hdr.vaddr, p.hdr.seqn});
+      addr_notes_.push_back(AddrNote{p.hdr.comm_sig, p.hdr.src, p.hdr.tag, p.hdr.count, p.hdr.vaddr, p.hdr.seqn, std::move(p.payload)});
       ++mailbox_events_;
       q_cv_.notify_all();
       break;

@@ -12,6 +12,7 @@
 // behaviours (resumable `Steps` instead of current_step gotos).
 #include <algorithm>
 #include <atomic>
+#include <cstring>
 
 #include "accl/common.hpp"
 #include "accl/cuda/plan.hpp" // the H100 backend's call planner (host / device shared, plain C++): one-hop schedule selection
@@ -55,7 +56,7 @@ bool Engine::elder_conflict(const EmuCall &c) {
   const bool p2p = op == operation::send || op == operation::recv;
   const bool coll = op == operation::bcast || op == operation::scatter || op == operation::gather || op == operation::allgather ||
                     op == operation::reduce || op == operation::reduce_scatter || op == operation::allreduce ||
-                    op == operation::alltoall;
+                    op == operation::alltoall || op == operation::alltoallv;
   if (!p2p && !coll) return false;
   std::lock_guard<std::mutex> g(q_m_);
   const size_t n = std::min(older_parked_, retry_calls_.size());
@@ -68,7 +69,8 @@ bool Engine::elder_conflict(const EmuCall &c) {
       if (eo == op && e.root_src_dst == c.desc.root_src_dst) return true;
     } else {
       if (eo == operation::bcast || eo == operation::scatter || eo == operation::gather || eo == operation::allgather ||
-          eo == operation::reduce || eo == operation::reduce_scatter || eo == operation::allreduce || eo == operation::alltoall)
+          eo == operation::reduce || eo == operation::reduce_scatter || eo == operation::allreduce || eo == operation::alltoall ||
+          eo == operation::alltoallv)
         return true;
     }
   }
@@ -96,6 +98,7 @@ uint32_t Engine::dispatch(EmuCall &c) {
   case operation::allreduce: return fw_allreduce(c);
   case operation::barrier: return fw_barrier(c);
   case operation::alltoall: return fw_alltoall(c);
+  case operation::alltoallv: return fw_alltoallv(c);
   }
   return COLLECTIVE_NOT_IMPLEMENTED;
 }
@@ -1212,6 +1215,125 @@ uint32_t Engine::fw_alltoall(EmuCall &c) {
     uint32_t from = 0;
     if (!rndzv_take_any_done(x, ((c.mask >> 16) & 0xFFFFu) | (1u << me), x.tag, from)) return NOT_READY_ERROR;
     c.mask |= 1u << (16 + from);
+  }
+  return 0;
+}
+
+// --------------------------------------------------------------- alltoallv
+// Beyond the reference.  Counts in memory at a1 (int64: P send counts, then P receive counts, in elements);
+// capacities in `count` (receive) and `root_src_dst` (send).  One exchange before any data moves: every rank
+// announces its receive buffer to every peer together with its whole count vector and its capacities, so each rank
+// checks the same matrix and reaches the same verdict (all-or-nothing: an invalid call writes nothing anywhere).
+// Then the blocks go straight into the receivers' buffers as one-sided writes, each followed by its completion
+// note.  The same schedule serves the eager and rendezvous sizes and the one-hop mode.
+uint32_t Engine::fw_alltoallv(EmuCall &c) {
+  FW_DECODE(x);
+  const uint32_t P = x.comm.size, me = x.comm.local_rank;
+  const uint64_t es = x.ubytes();
+  const size_t row_words = 2 * static_cast<size_t>(P) + 2; // counts, send capacity, receive capacity
+  auto my_row = [&] {
+    std::vector<int64_t> v(row_words, 0);
+    uint32_t e = 0;
+    const uint8_t *p = mem_ptr(x.a1, 2 * P * sizeof(int64_t), e);
+    if (p) std::memcpy(v.data(), p, 2 * P * sizeof(int64_t));
+    v[2 * P] = p ? static_cast<int64_t>(x.root) : -1; // unreadable counts: a negative capacity rejects the call
+    v[2 * P + 1] = static_cast<int64_t>(x.count);
+    return v;
+  };
+  Steps st(c.step);
+  st([&] {
+    const std::vector<int64_t> v = my_row();
+    for (uint32_t r = 0; r < P; ++r) {
+      if (r == me) continue;
+      Packet p;
+      p.hdr.msg_type = static_cast<uint32_t>(MsgType::RNDZVS_INIT);
+      p.hdr.src = static_cast<uint32_t>(rank_);
+      p.hdr.dst = x.comm.session[r];
+      p.hdr.tag = x.tag;
+      p.hdr.vaddr = x.a2;
+      p.hdr.comm_sig = x.comm.sig;
+      p.hdr.host = x.a2 >= HOST_BASE;
+      p.hdr.seqn = note_kind(x);
+      p.payload.resize(row_words * sizeof(int64_t));
+      std::memcpy(p.payload.data(), v.data(), p.payload.size());
+      fabric_->send(std::move(p));
+    }
+    return true;
+  });
+  uint32_t err = 0;
+  if (!st([&] {
+        // every peer's announcement, or none of them (a parked call keeps nothing but its step)
+        std::vector<std::vector<int64_t>> rows(P);
+        std::vector<uint64_t> dst_base(P, x.a2);
+        {
+          std::lock_guard<std::mutex> g(q_m_);
+          std::vector<std::list<AddrNote>::iterator> found(P, addr_notes_.end());
+          uint32_t n = 0;
+          for (auto it = addr_notes_.begin(); it != addr_notes_.end(); ++it) {
+            if (it->comm_sig != x.comm.sig || it->kind != note_kind(x)) continue;
+            for (uint32_t r = 0; r < P; ++r)
+              if (r != me && found[r] == addr_notes_.end() && x.comm.session[r] == it->src) {
+                found[r] = it;
+                ++n;
+                break;
+              }
+          }
+          if (n + 1 != P) return false;
+          for (uint32_t r = 0; r < P; ++r) {
+            if (r == me) continue;
+            rows[r].assign(row_words, -1);
+            if (found[r]->payload.size() == row_words * sizeof(int64_t))
+              std::memcpy(rows[r].data(), found[r]->payload.data(), found[r]->payload.size());
+            dst_base[r] = found[r]->vaddr;
+            addr_notes_.erase(found[r]);
+          }
+        }
+        rows[me] = my_row();
+        bool ok = true;
+        for (uint32_t p = 0; p < P && ok; ++p) { // each rank's own checks ...
+          const std::vector<int64_t> &v = rows[p];
+          int64_t s = 0, r = 0;
+          for (uint32_t q = 0; q < P && ok; ++q) {
+            ok = v[q] >= 0 && v[P + q] >= 0 && v[q] <= v[2 * P] && v[P + q] <= v[2 * P + 1];
+            s += ok ? v[q] : 0;
+            r += ok ? v[P + q] : 0;
+          }
+          ok = ok && s <= v[2 * P] && r <= v[2 * P + 1];
+        }
+        for (uint32_t p = 0; p < P && ok; ++p) // ... and every send count against its receiver's count
+          for (uint32_t q = 0; q < P && ok; ++q) ok = rows[p][q] == rows[q][P + p];
+        if (!ok) {
+          err = DMA_SIZE_ERROR;
+          return true;
+        }
+        uint64_t src_off = 0;
+        for (uint32_t q = 0; q < P; ++q) { // (after a failed write too: every peer gets its completion note)
+          uint64_t dst_off = 0; // after the blocks of q's lower senders
+          for (uint32_t p = 0; p < me; ++p) dst_off += static_cast<uint64_t>(rows[q][P + p]);
+          const uint32_t n = static_cast<uint32_t>(rows[me][q]);
+          if (q == me) {
+            if (n) {
+              Move m;
+              m.op0 = imm(x.a0 + src_off * es);
+              m.res = imm(x.a2 + dst_off * es);
+              m.count = n;
+              err |= execute(x, m);
+            }
+          } else {
+            err |= rndzv_write(x, q, x.a0 + src_off * es, dst_base[q] + dst_off * es, n, x.tag);
+          }
+          src_off += n;
+        }
+        return true;
+      }))
+    return NOT_READY_ERROR;
+  if (err) return err;
+  // only valid calls get here (an invalid one returned above on every rank): collect the completion notes
+  const uint32_t all = ((1u << P) - 1) & ~(1u << me);
+  while ((c.mask & all) != all) {
+    uint32_t from = 0;
+    if (!rndzv_take_any_done(x, c.mask | (1u << me), x.tag, from)) return NOT_READY_ERROR;
+    c.mask |= 1u << from;
   }
   return 0;
 }

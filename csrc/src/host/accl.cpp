@@ -171,6 +171,11 @@ void ACCL::configure_arithmetic() {
     kv.second.exchmem_addr = idx;
     ++idx;
   }
+  if (idx >= exchmem::MAX_ARITHCFG) throw std::runtime_error("too many arithmetic configurations");
+  uint32_t w[ARITHCFG_WORDS];
+  serialize_arithconfig(byte_move_config_, w);
+  for (int i = 0; i < ARITHCFG_WORDS; ++i) cclo->write(exchmem::arith_offset(idx, static_cast<uint32_t>(i)), w[i]);
+  byte_move_config_.exchmem_addr = idx++;
   cclo->write(exchmem::NUM_ARITHCFG, idx);
 }
 
@@ -284,7 +289,10 @@ void ACCL::prepare_call(CCLO::Options &o) {
   } else if (dtypes.size() == 1) {
     dataType t = *dtypes.begin();
     if (o.compress_dtype == dataType::none || o.compress_dtype == t) {
-      cfg = &arith_config.at({t, t});
+      const auto it = arith_config.find({t, t});
+      if (it != arith_config.end()) cfg = &it->second;
+      else if (o.scenario == operation::alltoallv && dtype_bytes(t) == 1) cfg = &byte_move_config_;
+      else cfg = &arith_config.at({t, t}); // (throws: no configuration for this type)
     } else {
       cfg = &arith_config.at({t, o.compress_dtype});
       o.compression_flags |= compressionFlags::ETH_COMPRESSED;
@@ -872,6 +880,36 @@ ACCLRequest *ACCL::alltoall(BaseBuffer &sendbuf, BaseBuffer &recvbuf, unsigned i
   o.waitfor = waitfor;
   ACCLRequest *h = call_async(o);
   ACCL_FINISH("alltoall", h, run_async, if (!to_fpga) r->sync_from_device());
+}
+
+ACCLRequest *ACCL::alltoallv(BaseBuffer &sendbuf, BaseBuffer &recvbuf, BaseBuffer &counts, communicatorId comm_id,
+                             bool from_fpga, bool to_fpga, bool run_async, std::vector<ACCLRequest *> waitfor) {
+  Communicator &c = comm(comm_id);
+  if (counts.type() != dataType::int64 || counts.length() < 2 * static_cast<size_t>(c.size()))
+    throw std::invalid_argument("alltoallv: counts must be an int64 buffer of at least 2 x communicator size elements");
+  if (counts.is_host_only() && cclo->get_device_type() == deviceType::cuda)
+    throw std::invalid_argument("alltoallv: counts must live in device memory (the engine reads them)");
+  if (sendbuf.type() != recvbuf.type()) throw std::invalid_argument("alltoallv: send and receive buffers differ in type");
+  // the capacities travel in 32-bit descriptor words: recv in `count`, send in `root_src_dst`
+  if (sendbuf.length() > 0xFFFFFFFFull || recvbuf.length() > 0xFFFFFFFFull)
+    throw std::invalid_argument("alltoallv: buffers longer than 2^32 - 1 elements");
+  if (!to_fpga && run_async) warn_async_sync("alltoallv");
+  if (!from_fpga) {
+    sendbuf.sync_to_device();
+    counts.sync_to_device();
+  }
+  CCLO::Options o;
+  o.scenario = operation::alltoallv;
+  o.comm = c.index();
+  o.addr_0 = &sendbuf;
+  o.addr_1 = &counts;
+  o.addr_2 = &recvbuf;
+  o.data_type_io_1 = sendbuf.type(); // the counts' own type does not select the arithmetic configuration
+  o.count = static_cast<unsigned int>(recvbuf.length());
+  o.root_src_dst = static_cast<unsigned int>(sendbuf.length());
+  o.waitfor = waitfor;
+  ACCLRequest *h = call_async(o);
+  ACCL_FINISH("alltoallv", h, run_async, if (!to_fpga) recvbuf.sync_from_device());
 }
 
 ACCLRequest *ACCL::barrier(communicatorId comm_id, std::vector<ACCLRequest *> waitfor) {

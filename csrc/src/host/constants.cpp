@@ -18,6 +18,7 @@ const char *operation_name(operation op) {
   case operation::reduce_scatter: return "reduce_scatter";
   case operation::barrier: return "barrier";
   case operation::alltoall: return "alltoall";
+  case operation::alltoallv: return "alltoallv";
   case operation::nop: return "nop";
   }
   return "unknown";
