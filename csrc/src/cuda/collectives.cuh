@@ -119,72 +119,77 @@ __device__ __noinline__ void op_combine(const Ctx &c) {
 }
 
 // ------------------------------------------------------------ eager slots
-struct EgrSeg { // one segment of one block, as seen by this CTA
-  size_t elem_off; // offset inside the block
-  uint32_t elems;
-};
+// The slot-ring handshake with one peer (global rank) on channel `ch`, per thread: message v from me to `peer` goes
+// into slot v % depth of my column of its ring, once the peer has handed back the credit for message v - depth; a
+// header describes it and the release of `egr_sig` announces it.  The counters, the header format and the slot
+// addressing are known only to these helpers.
+constexpr uint32_t EGR_LOST = 0xFFFFFFFFu; // egr_arrive: the message did not come in time
 
-__device__ __forceinline__ void egr_push(const Ctx &c, uint32_t peer_cr, const void *src, uint32_t src_t, uint32_t wire_t,
-                                          uint32_t elems, uint32_t tag, uint32_t *s_tmp) {
-  const uint32_t ch = static_cast<uint32_t>(c.cta);
-  const uint32_t peer = c.g(peer_cr);
-  __syncthreads(); // s_tmp may still be read by stragglers of the previous step
-  if (threadIdx.x == 0) {
-    const uint32_t v = c.me->egr_sent[ch][peer] + 1;
-    // credit: the slot I am about to overwrite (message v - depth) must have been consumed
-    if (v > c.w.egr_depth) wait_ge(&c.me->egr_ack[ch][peer], v - c.w.egr_depth, c, DEQUEUE_BUFFER_TIMEOUT_ERROR);
-    *s_tmp = v;
-  }
-  __syncthreads();
-  const uint32_t v = *s_tmp;
-  char *slot = c.heap(peer) + egr_slot_off(c.w, ch, v % c.w.egr_depth, c.w.rank);
-  cast_copy(slot, wire_t, src, src_t, elems, c.it.ratio_log);
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    Ctrl *pc = c.ctrl(peer);
-    EgrHdr *h = &pc->egr_hdr[ch][v % c.w.egr_depth][c.w.rank];
-    st_relaxed_sys(&h->tag, tag);
-    st_relaxed_sys(&h->bytes, static_cast<uint32_t>(wire_bytes(wire_t, c.it.ratio_log, elems)));
-    st_relaxed_sys(&h->elems, elems);
-    st_relaxed_sys(&h->kind, c.it.desc.scenario | (wire_t << 8));
-    st_release_sys(&pc->egr_sig[ch][c.w.rank], v);
-    c.me->egr_sent[ch][peer] = v;
-  }
+// may message sent + 1 be written? (its slot held message sent + 1 - depth, which must have been consumed)
+__device__ __forceinline__ bool egr_credit_ok(const Ctx &c, uint32_t ch, uint32_t peer) {
+  const uint32_t v = c.me->egr_sent[ch][peer] + 1;
+  return v <= c.w.egr_depth || static_cast<int32_t>(ld_acquire_sys(&c.me->egr_ack[ch][peer]) - (v - c.w.egr_depth)) >= 0;
 }
 
-// wait for the next message of `peer`; returns its payload (nullptr on timeout)
-__device__ __forceinline__ const char *egr_wait(const Ctx &c, uint32_t peer_cr, uint32_t want_tag, uint32_t want_elems,
-                                                 uint32_t wire_t, uint32_t *s_tmp) {
-  const uint32_t ch = static_cast<uint32_t>(c.cta);
-  const uint32_t peer = c.g(peer_cr);
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    const uint32_t e = c.me->egr_expect[ch][peer] + 1;
-    bool ok = wait_ge(&c.me->egr_sig[ch][peer], e, c, RECEIVE_TIMEOUT_ERROR);
-    if (ok) {
-      const EgrHdr *h = &c.me->egr_hdr[ch][e % c.w.egr_depth][peer];
-      const uint32_t tag = ld_relaxed_sys(&h->tag);
-      if (want_tag != TAG_ANY && tag != TAG_ANY && tag != want_tag) atomicOr(c.err, DMA_TAG_MISMATCH_ERROR);
-      if (ld_relaxed_sys(&h->elems) != want_elems) atomicOr(c.err, DMA_NOT_EXPECTED_BTT_ERROR);
-      if ((ld_relaxed_sys(&h->kind) >> 8) != wire_t) atomicOr(c.err, COMPRESSION_ERROR);
-    }
-    c.me->egr_expect[ch][peer] = e;
-    *s_tmp = ok ? e : 0xFFFFFFFFu;
+// wait for the credit of the next message; returns its number (DEQUEUE_BUFFER_TIMEOUT_ERROR on timeout)
+__device__ __forceinline__ uint32_t egr_credit_wait(const Ctx &c, uint32_t ch, uint32_t peer) {
+  const uint32_t v = c.me->egr_sent[ch][peer] + 1;
+  if (v > c.w.egr_depth) wait_ge(&c.me->egr_ack[ch][peer], v - c.w.egr_depth, c, DEQUEUE_BUFFER_TIMEOUT_ERROR);
+  return v;
+}
+
+// where message v to `peer` goes
+__device__ __forceinline__ char *egr_tx_slot(const Ctx &c, uint32_t ch, uint32_t peer, uint32_t v) {
+  return c.heap(peer) + egr_slot_off(c.w, ch, v % c.w.egr_depth, c.w.rank);
+}
+
+// Announce message v (its payload is in the slot): header, then the release of the arrival counter.  `fence` adds a
+// fence.acq_rel.sys between the two.  egr_collective asks for it, because other threads of its CTA wrote the payload.
+// egr_p2p's payload is written by the whole CTA as well, yet it has never issued the fence: the difference is
+// inherited, not derived, and is kept as it is.
+__device__ __forceinline__ void egr_publish(const Ctx &c, uint32_t ch, uint32_t peer, uint32_t v, uint32_t tag, uint32_t wire_t,
+                                            uint32_t elems, bool fence) {
+  Ctrl *pc = c.ctrl(peer);
+  EgrHdr *h = &pc->egr_hdr[ch][v % c.w.egr_depth][c.w.rank];
+  st_relaxed_sys(&h->tag, tag);
+  st_relaxed_sys(&h->bytes, static_cast<uint32_t>(wire_bytes(wire_t, c.it.ratio_log, elems)));
+  st_relaxed_sys(&h->elems, elems);
+  st_relaxed_sys(&h->kind, c.it.desc.scenario | (wire_t << 8));
+  if (fence) fence_acq_rel_sys();
+  st_release_sys(&pc->egr_sig[ch][c.w.rank], v);
+  c.me->egr_sent[ch][peer] = v;
+}
+
+// has the next message of `peer` arrived?
+__device__ __forceinline__ bool egr_arrived(const Ctx &c, uint32_t ch, uint32_t peer) {
+  return static_cast<int32_t>(ld_acquire_sys(&c.me->egr_sig[ch][peer]) - (c.me->egr_expect[ch][peer] + 1)) >= 0;
+}
+
+// Wait for the next message of `peer` and check its header against the tag, element count and wire dtype this call
+// expects.  Returns its number, or EGR_LOST on timeout; the message counts as consumed either way.
+__device__ __forceinline__ uint32_t egr_arrive(const Ctx &c, uint32_t ch, uint32_t peer, uint32_t want_tag, uint32_t want_elems,
+                                               uint32_t wire_t) {
+  const uint32_t e = c.me->egr_expect[ch][peer] + 1;
+  const bool ok = wait_ge(&c.me->egr_sig[ch][peer], e, c, RECEIVE_TIMEOUT_ERROR);
+  if (ok) {
+    const EgrHdr *h = &c.me->egr_hdr[ch][e % c.w.egr_depth][peer];
+    const uint32_t tag = ld_relaxed_sys(&h->tag);
+    if (want_tag != TAG_ANY && tag != TAG_ANY && tag != want_tag) atomicOr(c.err, DMA_TAG_MISMATCH_ERROR);
+    if (ld_relaxed_sys(&h->elems) != want_elems) atomicOr(c.err, DMA_NOT_EXPECTED_BTT_ERROR);
+    if ((ld_relaxed_sys(&h->kind) >> 8) != wire_t) atomicOr(c.err, COMPRESSION_ERROR);
   }
-  __syncthreads();
-  const uint32_t e = *s_tmp;
-  if (e == 0xFFFFFFFFu) return nullptr;
+  c.me->egr_expect[ch][peer] = e;
+  return ok ? e : EGR_LOST;
+}
+
+// where message e from `peer` is
+__device__ __forceinline__ const char *egr_rx_slot(const Ctx &c, uint32_t ch, uint32_t peer, uint32_t e) {
   return c.heap(c.w.rank) + egr_slot_off(c.w, ch, e % c.w.egr_depth, peer);
 }
 
-// all threads are done with the slot: hand the credit back to the sender
-__device__ __forceinline__ void egr_ack(const Ctx &c, uint32_t peer_cr) {
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    const uint32_t ch = static_cast<uint32_t>(c.cta);
-    const uint32_t peer = c.g(peer_cr);
-    st_relaxed_sys(&c.ctrl(peer)->egr_ack[ch][c.w.rank], c.me->egr_expect[ch][peer]);
-  }
+// the last consumed message of `peer` has been read out: hand its credit back
+__device__ __forceinline__ void egr_credit_return(const Ctx &c, uint32_t ch, uint32_t peer) {
+  st_relaxed_sys(&c.ctrl(peer)->egr_ack[ch][c.w.rank], c.me->egr_expect[ch][peer]);
 }
 
 // segment geometry shared by both ends: the block of `count` elements is cut
@@ -273,12 +278,7 @@ __device__ __noinline__ void egr_collective(const Ctx &c, Pattern pat, uint32_t 
     __syncthreads();
     if (t < ACCL_MAX_RANKS) s_slots[t] = nullptr;
     // ---- push phase: credits in parallel
-    if (t < P && ro.pushes_to(t)) {
-      const uint32_t peer = c.g(t);
-      const uint32_t v = c.me->egr_sent[ch][peer] + 1;
-      if (v > c.w.egr_depth) wait_ge(&c.me->egr_ack[ch][peer], v - c.w.egr_depth, c, DEQUEUE_BUFFER_TIMEOUT_ERROR);
-      s_v[t] = v;
-    }
+    if (t < P && ro.pushes_to(t)) s_v[t] = egr_credit_wait(c, ch, c.g(t));
     __syncthreads();
     if (same_src && src_t == wire_t && !is_fp8_dt(wire_t)) {
       // one read of my block, stores fan out to every destination slot
@@ -286,7 +286,7 @@ __device__ __noinline__ void egr_collective(const Ctx &c, Pattern pat, uint32_t 
       if (t == 0) {
         for (uint32_t k = 1; k < P; ++k) {
           const uint32_t q = (me + k) % P;
-          if (ro.pushes_to(q)) c.tab->dst[nd++] = c.heap(c.g(q)) + egr_slot_off(c.w, ch, s_v[q] % c.w.egr_depth, c.w.rank);
+          if (ro.pushes_to(q)) c.tab->dst[nd++] = egr_tx_slot(c, ch, c.g(q), s_v[q]);
         }
         c.tab->src[0] = src + e0 * se;
         *s_tmp = static_cast<uint32_t>(nd);
@@ -299,36 +299,16 @@ __device__ __noinline__ void egr_collective(const Ctx &c, Pattern pat, uint32_t 
         const uint32_t q = (me + k) % P; // stagger destinations across ranks
         if (!ro.pushes_to(q)) continue;
         const char *from = same_src ? src + e0 * se : src + (static_cast<size_t>(q) * count + e0) * se;
-        char *slot = c.heap(c.g(q)) + egr_slot_off(c.w, ch, s_v[q] % c.w.egr_depth, c.w.rank);
-        cast_copy(slot, wire_t, from, src_t, n, it.ratio_log);
+        cast_copy(egr_tx_slot(c, ch, c.g(q), s_v[q]), wire_t, from, src_t, n, it.ratio_log);
       }
     }
     __syncthreads();
-    if (t < P && ro.pushes_to(t)) { // headers + arrival flags in parallel
-      const uint32_t peer = c.g(t), v = s_v[t];
-      Ctrl *pc = c.ctrl(peer);
-      EgrHdr *h = &pc->egr_hdr[ch][v % c.w.egr_depth][c.w.rank];
-      st_relaxed_sys(&h->tag, tag);
-      st_relaxed_sys(&h->bytes, static_cast<uint32_t>(wire_bytes(wire_t, it.ratio_log, n)));
-      st_relaxed_sys(&h->elems, n);
-      st_relaxed_sys(&h->kind, it.desc.scenario | (wire_t << 8));
-      fence_acq_rel_sys(); // the payload was written by other threads of this CTA (ordered by the barrier above)
-      st_release_sys(&pc->egr_sig[ch][c.w.rank], v);
-      c.me->egr_sent[ch][peer] = v;
-    }
+    // headers + arrival flags in parallel; the payload was written by other threads of this CTA (ordered by the barrier above)
+    if (t < P && ro.pushes_to(t)) egr_publish(c, ch, c.g(t), s_v[t], tag, wire_t, n, true);
     // ---- wait phase: one thread per expected peer
     if (t < P && ro.expects_from(t)) {
-      const uint32_t peer = c.g(t);
-      const uint32_t e = c.me->egr_expect[ch][peer] + 1;
-      if (wait_ge(&c.me->egr_sig[ch][peer], e, c, RECEIVE_TIMEOUT_ERROR)) {
-        const EgrHdr *h = &c.me->egr_hdr[ch][e % c.w.egr_depth][peer];
-        const uint32_t htag = ld_relaxed_sys(&h->tag);
-        if (tag != TAG_ANY && htag != TAG_ANY && htag != tag) atomicOr(c.err, DMA_TAG_MISMATCH_ERROR);
-        if (ld_relaxed_sys(&h->elems) != n) atomicOr(c.err, DMA_NOT_EXPECTED_BTT_ERROR);
-        if ((ld_relaxed_sys(&h->kind) >> 8) != wire_t) atomicOr(c.err, COMPRESSION_ERROR);
-        s_slots[t] = c.heap(c.w.rank) + egr_slot_off(c.w, ch, e % c.w.egr_depth, peer);
-      }
-      c.me->egr_expect[ch][peer] = e;
+      const uint32_t peer = c.g(t), e = egr_arrive(c, ch, peer, tag, n, wire_t);
+      if (e != EGR_LOST) s_slots[t] = egr_rx_slot(c, ch, peer, e);
     }
     __syncthreads();
     bool ok = *c.err == 0;
@@ -367,41 +347,52 @@ __device__ __noinline__ void egr_collective(const Ctx &c, Pattern pat, uint32_t 
     }
     // ---- credits back to the senders
     __syncthreads();
-    if (t < P && s_slots[t]) st_relaxed_sys(&c.ctrl(c.g(t))->egr_ack[ch][c.w.rank], c.me->egr_expect[ch][c.g(t)]);
+    if (t < P && s_slots[t]) egr_credit_return(c, ch, c.g(t));
   }
   __syncthreads();
 }
 
-// eager point-to-point (channel 0 only)
-__device__ __noinline__ void egr_send(const Ctx &c, uint32_t *s_tmp) {
+// Eager point-to-point: CTA 0 moves the message segment by segment through channel 0 of the slot ring, its thread 0
+// keeps the handshake.  Starts `progress` elements in and returns how far it got: the element count when done (or when
+// a segment did not arrive in time, with the error set).  `park`: return early instead of blocking at the first
+// missing credit (send) or segment (recv), so that the engine can step other calls and come back.
+__device__ __noinline__ unsigned long long egr_p2p(const Ctx &c, bool sending, bool park, unsigned long long progress, uint32_t *s_tmp) {
   const WorkItem &it = c.it;
-  if (c.cta != 0) return;
+  if (c.cta != 0) return progress;
   const uint32_t cf = it.desc.compression_flags;
-  const uint32_t src_t = (cf & 1) ? it.cdtype : it.udtype, wire_t = (cf & 8) ? it.cdtype : it.udtype;
-  const char *src = c.heap(c.w.rank) + it.desc.addr0();
+  const uint32_t src_t = (cf & 1) ? it.cdtype : it.udtype, dst_t = (cf & 4) ? it.cdtype : it.udtype;
+  const uint32_t wire_t = (cf & 8) ? it.cdtype : it.udtype;
+  const uint32_t peer = c.g(it.desc.root_src_dst);
+  const unsigned long long count = it.desc.count;
   const uint32_t seg = egr_seg_elems(c, wire_t);
-  for (size_t off = 0; off < it.desc.count; off += seg) {
-    const uint32_t n = static_cast<uint32_t>(it.desc.count - off < seg ? it.desc.count - off : seg);
-    egr_push(c, it.desc.root_src_dst, src + off * esize(src_t), src_t, wire_t, n, it.desc.tag, s_tmp);
+  while (progress < count) {
+    const uint32_t n = static_cast<uint32_t>(count - progress < seg ? count - progress : seg);
+    __syncthreads(); // s_tmp may still be read by stragglers of the previous step
+    if (park) {
+      if (threadIdx.x == 0) *s_tmp = sending ? egr_credit_ok(c, 0, peer) : egr_arrived(c, 0, peer);
+      __syncthreads();
+      if (!*s_tmp) return progress;
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) *s_tmp = sending ? egr_credit_wait(c, 0, peer) : egr_arrive(c, 0, peer, it.desc.tag, n, wire_t);
     __syncthreads();
-  }
-}
-
-__device__ __noinline__ void egr_recv(const Ctx &c, uint32_t *s_tmp) {
-  const WorkItem &it = c.it;
-  if (c.cta != 0) return;
-  const uint32_t cf = it.desc.compression_flags;
-  const uint32_t dst_t = (cf & 4) ? it.cdtype : it.udtype, wire_t = (cf & 8) ? it.cdtype : it.udtype;
-  char *dst = c.heap(c.w.rank) + it.desc.addr2();
-  const uint32_t seg = egr_seg_elems(c, wire_t);
-  for (size_t off = 0; off < it.desc.count; off += seg) {
-    const uint32_t n = static_cast<uint32_t>(it.desc.count - off < seg ? it.desc.count - off : seg);
-    const char *sp = egr_wait(c, it.desc.root_src_dst, it.desc.tag, n, wire_t, s_tmp);
-    if (!sp) return;
-    cast_copy(dst + off * esize(dst_t), dst_t, sp, wire_t, n, it.ratio_log);
-    egr_ack(c, it.desc.root_src_dst);
+    const uint32_t v = *s_tmp;
+    if (sending) {
+      cast_copy(egr_tx_slot(c, 0, peer, v), wire_t, c.heap(c.w.rank) + it.desc.addr0() + progress * esize(src_t), src_t, n,
+                it.ratio_log);
+      __syncthreads();
+      if (threadIdx.x == 0) egr_publish(c, 0, peer, v, it.desc.tag, wire_t, n, false);
+    } else {
+      if (v == EGR_LOST) return count;
+      cast_copy(c.heap(c.w.rank) + it.desc.addr2() + progress * esize(dst_t), dst_t, egr_rx_slot(c, 0, peer, v), wire_t, n,
+                it.ratio_log);
+      __syncthreads();
+      if (threadIdx.x == 0) egr_credit_return(c, 0, peer);
+    }
     __syncthreads();
+    progress += n;
   }
+  return progress;
 }
 
 // ------------------------------------------------------ rendezvous bodies

@@ -70,6 +70,14 @@ __device__ __forceinline__ Ctrl *my_ctrl(const DevWorld &w) {
   return reinterpret_cast<Ctrl *>(w.window + static_cast<uint64_t>(w.rank) * w.heap_bytes);
 }
 
+// copy a WorkItem or MoveDesc as 8-byte words, with threads [0, stride) of the caller (the CTA or one warp)
+template <typename T> __device__ __forceinline__ void copy_words(T *dst, const T *src, uint32_t stride) {
+  static_assert(sizeof(T) % 8 == 0, "copied as whole 8-byte words");
+  const unsigned long long *s = reinterpret_cast<const unsigned long long *>(src);
+  unsigned long long *d = reinterpret_cast<unsigned long long *>(dst);
+  for (uint32_t i = threadIdx.x; i < sizeof(T) / 8; i += stride) d[i] = s[i];
+}
+
 // ------------------------------------------------------------------ workers
 // Move i is complete when all `nworkers` CTAs have passed it (participants after executing their share).
 __device__ void engine_worker(const DevWorld &w, int nworkers) {
@@ -99,11 +107,7 @@ __device__ void engine_worker(const DevWorld &w, int nworkers) {
     __syncthreads();
     if (s_exit) return;
     const uint32_t slot = static_cast<uint32_t>(next % MOVE_SLOTS);
-    {
-      const unsigned long long *src = reinterpret_cast<const unsigned long long *>(&ea->move_ring[slot]);
-      unsigned long long *dst = reinterpret_cast<unsigned long long *>(&s_mv);
-      for (uint32_t i = threadIdx.x; i < sizeof(MoveDesc) / 8; i += blockDim.x) dst[i] = src[i];
-    }
+    copy_words(&s_mv, &ea->move_ring[slot], blockDim.x);
     __syncthreads();
     const int nctas = static_cast<int>(s_mv.n_ctas);
     if (static_cast<int>(blockIdx.x) < nctas) {
@@ -186,14 +190,10 @@ __device__ bool move_issue(const EngCtx &e, Call &cl, uint32_t kind, uint32_t n_
   ok = bcast0(e, ok);
   if (!ok) return false;
   MoveDesc *mv = &e.ea->move_ring[slot];
-  {
-    const unsigned long long *src = reinterpret_cast<const unsigned long long *>(&cl.item);
-    unsigned long long *dst = reinterpret_cast<unsigned long long *>(&mv->item);
-    for (uint32_t i = threadIdx.x; i < sizeof(WorkItem) / 8; i += blockDim.x) dst[i] = src[i];
-    if (threadIdx.x < ACCL_MAX_RANKS) {
-      mv->off0[threadIdx.x] = cl.off0[threadIdx.x];
-      mv->off2[threadIdx.x] = cl.off2[threadIdx.x];
-    }
+  copy_words(&mv->item, &cl.item, blockDim.x);
+  if (threadIdx.x < ACCL_MAX_RANKS) {
+    mv->off0[threadIdx.x] = cl.off0[threadIdx.x];
+    mv->off2[threadIdx.x] = cl.off2[threadIdx.x];
   }
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -229,56 +229,38 @@ __device__ bool move_finished(const EngCtx &e, Call &cl) {
 // ---- rendezvous meetings on the engine's own channel of the call's bank, split into post and poll
 constexpr int ENG_CH = MAX_CH - 2; // (MAX_CH - 1 belongs to the GEMM plugin)
 
+// the call as the device helpers see it (one CTA; the meetings name their channel themselves)
+__device__ __forceinline__ k::Ctx call_ctx(const EngCtx &e, const Call &cl, uint32_t *err) {
+  return k::Ctx{e.w, cl.item, 0, 1, e.me, err, static_cast<uint64_t>(cl.item.timeout_us) * 1000ull, nullptr};
+}
+
 __device__ void meet_post(const EngCtx &e, Call &cl, bool exchange, uint64_t off0, uint64_t off2) {
-  const WorkItem &it = cl.item;
+  const k::Ctx c = call_ctx(e, cl, &cl.err);
   __syncthreads();
   const uint32_t t = threadIdx.x;
-  if (t < it.comm_size) {
-    const uint32_t peer = it.members[t];
-    if (t == it.comm_rank) {
-      cl.off0[t] = off0;
-      cl.off2[t] = off2;
-    } else {
-      PadBank &mine = e.me->pad[it.bank];
-      PadBank &theirs = reinterpret_cast<Ctrl *>(e.w.window + static_cast<uint64_t>(peer) * e.w.heap_bytes)->pad[it.bank];
-      const uint32_t v = mine.sent[ENG_CH][peer] + 1;
-      mine.sent[ENG_CH][peer] = v;
-      if (exchange) {
-        SyncRec *rr = &theirs.rec[ENG_CH][e.w.rank];
-        dev::st_relaxed_sys(&rr->off0, off0);
-        dev::st_relaxed_sys(&rr->off2, off2);
-        dev::st_relaxed_sys(&rr->kind, (it.desc.scenario & 0xFFu) | (it.comm_sig << 8));
-      }
-      dev::st_release_sys(&theirs.sig[ENG_CH][e.w.rank], v);
-    }
+  if (t == c.r()) {
+    cl.off0[t] = off0;
+    cl.off2[t] = off2;
+  } else if (t < c.P()) {
+    k::pad_post(c, ENG_CH, c.g(t), exchange ? k::REC_OFFS : k::REC_NONE, off0, off2, c.kind_word());
   }
   __syncthreads();
 }
 
-// true once every member has posted its side of the meeting (then the offsets are in cl.off0 / off2)
+// true once every member has posted its side of the meeting (then the offsets are in cl.off0 / off2).  All or
+// nothing: no post is taken before every peer's has arrived, so a parked meeting is polled again from scratch.
 __device__ bool meet_poll(const EngCtx &e, Call &cl, bool exchange) {
-  const WorkItem &it = cl.item;
+  const k::Ctx c = call_ctx(e, cl, &cl.err);
   const uint32_t t = threadIdx.x;
-  __syncthreads();
-  if (t == 0) *e.s_flag = 1;
-  __syncthreads();
-  if (t < it.comm_size && t != it.comm_rank) {
-    const uint32_t peer = it.members[t];
-    PadBank &mine = e.me->pad[it.bank];
-    if (static_cast<int32_t>(dev::ld_acquire_sys(&mine.sig[ENG_CH][peer]) - (mine.expect[ENG_CH][peer] + 1)) < 0) *e.s_flag = 0;
-  }
-  __syncthreads();
-  const bool all = *e.s_flag != 0;
-  __syncthreads();
-  if (all && t < it.comm_size && t != it.comm_rank) {
-    const uint32_t peer = it.members[t];
-    PadBank &mine = e.me->pad[it.bank];
-    mine.expect[ENG_CH][peer] += 1;
+  const bool peer = t < c.P() && t != c.r();
+  const bool all = __syncthreads_and(!peer || k::pad_arrived(c, ENG_CH, c.g(t))) != 0;
+  if (all && peer) {
+    k::pad_take(c, ENG_CH, c.g(t));
     if (exchange) {
-      const SyncRec *mr = &mine.rec[ENG_CH][peer];
-      cl.off0[t] = dev::ld_relaxed_sys(&mr->off0);
-      cl.off2[t] = dev::ld_relaxed_sys(&mr->off2);
-      if (dev::ld_relaxed_sys(&mr->kind) != ((it.desc.scenario & 0xFFu) | (it.comm_sig << 8))) atomicOr(&cl.err, PACK_SEQ_NUMBER_ERROR);
+      const SyncRec r = k::pad_rec(c, ENG_CH, c.g(t), k::REC_OFFS);
+      cl.off0[t] = r.off0;
+      cl.off2[t] = r.off2;
+      if (r.kind != c.kind_word()) atomicOr(c.err, PACK_SEQ_NUMBER_ERROR);
     }
   }
   __syncthreads();
@@ -290,7 +272,6 @@ __device__ uint32_t step_call(const EngCtx &e, Call &cl, uint32_t *s_err) {
   const WorkItem &it = cl.item;
   const operation op = static_cast<operation>(it.desc.scenario);
   const uint32_t t = threadIdx.x;
-  const uint64_t timeout_ns = static_cast<uint64_t>(it.timeout_us) * 1000ull;
   char *heap = e.w.window + static_cast<uint64_t>(e.w.rank) * e.w.heap_bytes;
 
   if (op == operation::nop || op == operation::config) return SR_DONE;
@@ -310,38 +291,12 @@ __device__ uint32_t step_call(const EngCtx &e, Call &cl, uint32_t *s_err) {
     const uint32_t peer_cr = it.desc.root_src_dst;
     const uint32_t peer = it.members[peer_cr];
     Ctrl *pc = reinterpret_cast<Ctrl *>(e.w.window + static_cast<uint64_t>(peer) * e.w.heap_bytes);
-    const uint32_t cf = it.desc.compression_flags;
     if (it.algo == ALGO_EAGER) {
-      // eager: segment by segment through the slot ring of channel 0; a missing credit (sender) or a message
-      // that has not arrived yet (receiver) parks the call with `progress` = elements already transferred
-      const uint32_t src_t = (cf & 1) ? it.cdtype : it.udtype, dst_t = (cf & 4) ? it.cdtype : it.udtype;
-      const uint32_t wire_t = (cf & 8) ? it.cdtype : it.udtype;
-      k::Ctx c{e.w, it, 0, 1, e.me, s_err, timeout_ns, nullptr};
-      const uint32_t seg = k::egr_seg_elems(c, wire_t);
-      while (cl.progress < it.desc.count) {
-        const uint32_t n = static_cast<uint32_t>(it.desc.count - cl.progress < seg ? it.desc.count - cl.progress : seg);
-        uint32_t ready = 0;
-        if (t == 0) {
-          if (sending) {
-            const uint32_t v = e.me->egr_sent[0][peer] + 1;
-            ready = v <= e.w.egr_depth || static_cast<int32_t>(dev::ld_acquire_sys(&e.me->egr_ack[0][peer]) - (v - e.w.egr_depth)) >= 0;
-          } else {
-            ready = static_cast<int32_t>(dev::ld_acquire_sys(&e.me->egr_sig[0][peer]) - (e.me->egr_expect[0][peer] + 1)) >= 0;
-          }
-        }
-        if (!bcast0(e, ready)) return SR_NOT_READY;
-        if (sending) {
-          k::egr_push(c, peer_cr, heap + it.desc.addr0() + cl.progress * k::esize(src_t), src_t, wire_t, n, it.desc.tag, e.s_flag);
-        } else {
-          const char *sp = k::egr_wait(c, peer_cr, it.desc.tag, n, wire_t, e.s_flag);
-          if (sp) k::cast_copy(heap + it.desc.addr2() + cl.progress * k::esize(dst_t), dst_t, sp, wire_t, n, it.ratio_log);
-          k::egr_ack(c, peer_cr);
-        }
-        __syncthreads();
-        if (t == 0) cl.progress += n;
-        __syncthreads();
-      }
-      return SR_DONE;
+      // a missing credit (sender) or a segment that has not arrived yet (receiver) parks the call with `progress`
+      const unsigned long long done = k::egr_p2p(call_ctx(e, cl, s_err), sending, true, cl.progress, e.s_flag);
+      __syncthreads();
+      if (t == 0) cl.progress = done;
+      return done < it.desc.count ? SR_NOT_READY : SR_DONE;
     }
     // rendezvous through the address mailbox
     if (!sending) {
@@ -523,11 +478,7 @@ __device__ void engine_control(const DevWorld &w, HostRing *hr, int nworkers) {
       uint32_t slot = 0;
       while (s_calls[slot].active) ++slot;
       Call &cl = s_calls[slot];
-      {
-        const unsigned long long *src = reinterpret_cast<const unsigned long long *>(&ea->cmd_ring[fetched % RING_SLOTS].item);
-        unsigned long long *dst = reinterpret_cast<unsigned long long *>(&cl.item);
-        for (uint32_t i = t; i < sizeof(WorkItem) / 8; i += blockDim.x) dst[i] = src[i];
-      }
+      copy_words(&cl.item, &ea->cmd_ring[fetched % RING_SLOTS].item, blockDim.x);
       __syncthreads();
       if (t == 0) {
         cl.err = 0;
@@ -676,9 +627,7 @@ __global__ void __launch_bounds__(32) k_submit(DevWorld w, WorkItem item, int wa
     }
   }
   t = __shfl_sync(0xffffffffu, t, 0);
-  const unsigned long long *src = reinterpret_cast<const unsigned long long *>(&item);
-  unsigned long long *dst = reinterpret_cast<unsigned long long *>(&ea->cmd_ring[t % RING_SLOTS].item);
-  for (uint32_t i = threadIdx.x; i < sizeof(WorkItem) / 8; i += 32) dst[i] = src[i];
+  copy_words(&ea->cmd_ring[t % RING_SLOTS].item, &item, 32);
   __syncwarp();
   if (threadIdx.x == 0) {
     __threadfence();

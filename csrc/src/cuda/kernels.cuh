@@ -69,6 +69,62 @@ __device__ __forceinline__ bool wait_ge(const uint32_t *p, uint32_t target, cons
   return true;
 }
 
+// ------------------------------------------------------ sync-pad meetings
+// A meeting of this rank with one peer on channel `ch` of the call's bank (global rank `peer`): each side posts
+// (sent += 1, optionally a record, then the release of the peer's `sig`), then takes the peer's post (expect += 1)
+// once `sig` has reached it.  The pad layout and the record format are known only to the helpers below.  They are
+// per thread and never call __syncthreads: a CTA serves its peers with one thread each, the GEMM plugin with one lane
+// each, and the engine polls with `pad_arrived` instead of blocking.
+
+// which fields of the record a post carries: none (a bare signal), off0 + kind, or off0 + off2 + kind
+enum PadRec : uint32_t { REC_NONE, REC_OFF0, REC_OFFS };
+
+__device__ __forceinline__ void pad_post(const Ctx &c, uint32_t ch, uint32_t peer, PadRec rec, uint64_t off0, uint64_t off2,
+                                         uint32_t kind) {
+  PadBank &mine = c.pads();
+  PadBank &theirs = c.pads_of(peer);
+  const uint32_t v = mine.sent[ch][peer] + 1;
+  mine.sent[ch][peer] = v;
+  if (rec != REC_NONE) {
+    SyncRec *rr = &theirs.rec[ch][c.w.rank];
+    st_relaxed_sys(&rr->off0, off0);
+    if (rec == REC_OFFS) st_relaxed_sys(&rr->off2, off2);
+    st_relaxed_sys(&rr->kind, kind);
+  }
+  st_release_sys(&theirs.sig[ch][c.w.rank], v);
+}
+
+// has the peer's next post landed?
+__device__ __forceinline__ bool pad_arrived(const Ctx &c, uint32_t ch, uint32_t peer) {
+  const PadBank &mine = c.pads();
+  return static_cast<int32_t>(ld_acquire_sys(&mine.sig[ch][peer]) - (mine.expect[ch][peer] + 1)) >= 0;
+}
+
+// take the peer's next post (after pad_arrived); returns its number
+__device__ __forceinline__ uint32_t pad_take(const Ctx &c, uint32_t ch, uint32_t peer) {
+  PadBank &mine = c.pads();
+  const uint32_t e = mine.expect[ch][peer] + 1;
+  mine.expect[ch][peer] = e;
+  return e;
+}
+
+// take the peer's next post and wait for it; false + RECEIVE_TIMEOUT_ERROR on timeout.  The post counts as taken
+// either way, so the next meeting waits for the peer's next post.
+__device__ __forceinline__ bool pad_wait(const Ctx &c, uint32_t ch, uint32_t peer) {
+  const uint32_t e = pad_take(c, ch, peer);
+  return wait_ge(&c.pads().sig[ch][peer], e, c, RECEIVE_TIMEOUT_ERROR);
+}
+
+// the record of the post just taken, as far as `rec` says the peer wrote it
+__device__ __forceinline__ SyncRec pad_rec(const Ctx &c, uint32_t ch, uint32_t peer, PadRec rec) {
+  const SyncRec *mr = &c.pads().rec[ch][peer];
+  SyncRec r{};
+  r.off0 = ld_relaxed_sys(&mr->off0);
+  if (rec == REC_OFFS) r.off2 = ld_relaxed_sys(&mr->off2);
+  r.kind = ld_relaxed_sys(&mr->kind);
+  return r;
+}
+
 // Symmetric synchronisation of this CTA's channel with the same channel of
 // every communicator peer.  Optionally carries (off0, off2) to the peers —
 // the rendezvous address exchange — and returns theirs in shared arrays.
@@ -78,34 +134,20 @@ __device__ __forceinline__ void chan_sync(const Ctx &c, bool exchange, uint64_t 
   __syncthreads(); // every thread's prior writes happen-before the release below
   const uint32_t t = threadIdx.x;
   const uint32_t ch = static_cast<uint32_t>(c.cta);
-  if (t < c.P()) {
+  if (t == c.r()) {
+    if (exchange) {
+      s_off0[t] = my_off0;
+      s_off2[t] = my_off2;
+    }
+  } else if (t < c.P()) {
     const uint32_t peer = c.g(t);
-    if (t == c.r()) {
-      if (exchange) {
-        s_off0[t] = my_off0;
-        s_off2[t] = my_off2;
-      }
-    } else {
-      PadBank &mine = c.pads();
-      PadBank &theirs = c.pads_of(peer);
-      const uint32_t v = mine.sent[ch][peer] + 1;
-      mine.sent[ch][peer] = v;
-      if (exchange) {
-        SyncRec *rr = &theirs.rec[ch][c.w.rank];
-        st_relaxed_sys(&rr->off0, my_off0);
-        st_relaxed_sys(&rr->off2, my_off2);
-        st_relaxed_sys(&rr->kind, c.kind_word());
-      }
-      st_release_sys(&theirs.sig[ch][c.w.rank], v);
-      const uint32_t e = mine.expect[ch][peer] + 1;
-      mine.expect[ch][peer] = e;
-      if (wait_ge(&mine.sig[ch][peer], e, c, RECEIVE_TIMEOUT_ERROR) && exchange) {
-        const SyncRec *mr = &mine.rec[ch][peer];
-        s_off0[t] = ld_relaxed_sys(&mr->off0);
-        s_off2[t] = ld_relaxed_sys(&mr->off2);
-        // a peer in a different operation, or in a different communicator that hashes onto this bank
-        if (ld_relaxed_sys(&mr->kind) != c.kind_word()) atomicOr(c.err, PACK_SEQ_NUMBER_ERROR);
-      }
+    pad_post(c, ch, peer, exchange ? REC_OFFS : REC_NONE, my_off0, my_off2, c.kind_word());
+    if (pad_wait(c, ch, peer) && exchange) {
+      const SyncRec r = pad_rec(c, ch, peer, REC_OFFS);
+      s_off0[t] = r.off0;
+      s_off2[t] = r.off2;
+      // a peer in a different operation, or in a different communicator that hashes onto this bank
+      if (r.kind != c.kind_word()) atomicOr(c.err, PACK_SEQ_NUMBER_ERROR);
     }
   }
   __syncthreads();
@@ -120,22 +162,11 @@ __device__ __forceinline__ void pair_sync(const Ctx &c, uint32_t peer_comm_rank,
   if (threadIdx.x == 0) {
     const uint32_t ch = static_cast<uint32_t>(c.cta);
     const uint32_t peer = c.g(peer_comm_rank);
-    PadBank &mine = c.pads();
-    PadBank &theirs = c.pads_of(peer);
-    const uint32_t v = mine.sent[ch][peer] + 1;
-    mine.sent[ch][peer] = v;
-    if (post_rec) {
-      SyncRec *rr = &theirs.rec[ch][c.w.rank];
-      st_relaxed_sys(&rr->off0, my_off);
-      st_relaxed_sys(&rr->kind, my_kind);
-    }
-    st_release_sys(&theirs.sig[ch][c.w.rank], v);
-    const uint32_t e = mine.expect[ch][peer] + 1;
-    mine.expect[ch][peer] = e;
-    if (wait_ge(&mine.sig[ch][peer], e, c, RECEIVE_TIMEOUT_ERROR)) {
-      const SyncRec *mr = &mine.rec[ch][peer];
-      *peer_off = ld_relaxed_sys(&mr->off0);
-      *peer_kind = ld_relaxed_sys(&mr->kind);
+    pad_post(c, ch, peer, post_rec ? REC_OFF0 : REC_NONE, my_off, 0, my_kind);
+    if (pad_wait(c, ch, peer)) {
+      const SyncRec r = pad_rec(c, ch, peer, REC_OFF0);
+      *peer_off = r.off0;
+      *peer_kind = r.kind;
     } else {
       *peer_off = INVALID_OFF;
       *peer_kind = 0xFFFFFFFFu;

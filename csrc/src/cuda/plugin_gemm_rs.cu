@@ -334,21 +334,11 @@ k_plugin_gemm_rs(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       __threadfence();
       uint64_t peer_off = p.out_off;
       if (static_cast<uint32_t>(lane) < P && static_cast<uint32_t>(lane) != me) {
-        PadBank &mine = ctx.pads();
-        PadBank &theirs = ctx.pads_of(lane);
-        const uint32_t ch = MAX_CH - 1;
-        const uint32_t v = mine.sent[ch][lane] + 1;
-        mine.sent[ch][lane] = v;
-        SyncRec *rr = &theirs.rec[ch][me];
-        dev::st_relaxed_sys(&rr->off0, p.out_off);
-        dev::st_relaxed_sys(&rr->off2, p.out_off);
-        dev::st_relaxed_sys(&rr->kind, ctx.kind_word());
-        dev::st_release_sys(&theirs.sig[ch][me], v);
-        const uint32_t e = mine.expect[ch][lane] + 1;
-        mine.expect[ch][lane] = e;
-        if (k::wait_ge(&mine.sig[ch][lane], e, ctx, RECEIVE_TIMEOUT_ERROR)) {
-          peer_off = dev::ld_relaxed_sys(&mine.rec[ch][lane].off0);
-          if (dev::ld_relaxed_sys(&mine.rec[ch][lane].kind) != ctx.kind_word()) atomicOr(&s_err, PACK_SEQ_NUMBER_ERROR);
+        k::pad_post(ctx, MAX_CH - 1, lane, k::REC_OFFS, p.out_off, p.out_off, ctx.kind_word());
+        if (k::pad_wait(ctx, MAX_CH - 1, lane)) {
+          const SyncRec r = k::pad_rec(ctx, MAX_CH - 1, lane, k::REC_OFF0);
+          peer_off = r.off0;
+          if (r.kind != ctx.kind_word()) atomicOr(&s_err, PACK_SEQ_NUMBER_ERROR);
         }
       }
       if (static_cast<uint32_t>(lane) < P) reinterpret_cast<volatile uint64_t *>(p.grid_flags + 8)[lane] = peer_off;

@@ -61,11 +61,11 @@ __device__ __noinline__ void run_work(const DevWorld &w, const WorkItem &it, int
   case operation::copy: op_copy(c); return;
   case operation::combine: op_combine(c); return;
   case operation::send:
-    if (eager) egr_send(c, &s_tmp);
+    if (eager) egr_p2p(c, true, false, 0, &s_tmp);
     else rv_send(c, s_off0);
     return;
   case operation::recv:
-    if (eager) egr_recv(c, &s_tmp);
+    if (eager) egr_p2p(c, false, false, 0, &s_tmp);
     else rv_recv(c, s_off0);
     return;
   case operation::barrier:
