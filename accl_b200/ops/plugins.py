@@ -4,6 +4,9 @@
   K-slice on the tensor cores (wgmma) and each finished tile is added straight
   into the owner rank's output shard over NVLink (no intermediate C, no
   separate reduce_scatter kernel).
+* all_gather_gemm: the column-parallel counterpart — the GEMM starts on this
+  rank's own rows while the kernel pulls the peers' shards over NVLink, and
+  each peer tile waits only for its own 128 rows.
 * vadd_allreduce: the vector-add plugin; the kernel computes x + y chunk by
   chunk and hands every finished chunk to the persistent engine itself
   (device API, all_reduce_async) while it computes the next one.
@@ -41,6 +44,63 @@ def gemm_reduce_scatter(accl: Accl, a: torch.Tensor, w: torch.Tensor, out: Buffe
     assert out.length >= M // P * N
     _C.gemm_reduce_scatter(accl.impl, a.data_ptr(), w.data_ptr(), out.impl, M, N, K, _stream_handle(accl), variant)
     return out
+
+
+def _check_operand(name, t, device):
+    if not isinstance(t, torch.Tensor) or t.device != device:
+        raise ValueError(f"all_gather_gemm: {name} must be a tensor on {device}")
+    if t.dtype != torch.bfloat16 or t.dim() != 2 or not t.is_contiguous():
+        raise ValueError(f"all_gather_gemm: {name} must be a contiguous 2-D bf16 tensor, got {t.dtype} {tuple(t.shape)}")
+
+
+def _overlap(a: torch.Tensor, b: torch.Tensor) -> bool:
+    a0, b0 = a.data_ptr(), b.data_ptr()
+    return a0 < b0 + b.numel() * b.element_size() and b0 < a0 + a.numel() * a.element_size()
+
+
+def all_gather_gemm(accl: Accl, a_shard: torch.Tensor, w: torch.Tensor, out: torch.Tensor = None,
+                    gathered: torch.Tensor = None, status: torch.Tensor = None):
+    """out[M, N] = all_gather over ranks of a_shard[M/P, K], times w[N, K]^T.  Returns (out, gathered).
+
+    `a_shard` is this rank's rows, a contiguous bf16 tensor in the symmetric heap (a `Buffer.dev` view or a tensor
+    from `heap_mem_pool()`), at the same heap offset on every rank: allocate it in the same order everywhere.
+    `w` is this rank's output features (bf16, nn.Linear layout).  `out` (bf16 [M, N]) and `gathered` (bf16 [M, K],
+    every rank's shard in rank order) are ordinary CUDA tensors, allocated when not given.  Needs M % (128 * P) == 0,
+    N % 256 == 0, K % 64 == 0 and M <= 128 * 1024.  Stream ordered: a rank may rewrite its shard on the stream right
+    after the call.
+    `status`, optional 1-element int32 CUDA tensor, receives the error bits when the kernel ends (0: success); a
+    shard at a different heap offset on some peer sets DMA_MISMATCH_ERROR (bit 0) on both ranks and is not read.
+    Raises ValueError for a shard outside the heap, a wrong dtype, shape or layout, or `out` / `gathered` overlapping
+    the shard or each other."""
+    if not isinstance(a_shard, torch.Tensor) or not accl.heap_contains(a_shard):
+        raise ValueError("all_gather_gemm: a_shard must live in the symmetric heap (a Buffer.dev view or a heap_mem_pool tensor)")
+    device = a_shard.device
+    _check_operand("a_shard", a_shard, device)
+    _check_operand("w", w, device)
+    m, K = a_shard.shape
+    M, N = m * accl.world, w.shape[0]
+    if w.shape[1] != K:
+        raise ValueError(f"all_gather_gemm: w has K = {w.shape[1]}, a_shard has K = {K}")
+    if out is None:
+        out = torch.empty(M, N, dtype=torch.bfloat16, device=device)
+    if gathered is None:
+        gathered = torch.empty(M, K, dtype=torch.bfloat16, device=device)
+    _check_operand("out", out, device)
+    _check_operand("gathered", gathered, device)
+    if tuple(out.shape) != (M, N) or tuple(gathered.shape) != (M, K):
+        raise ValueError(f"all_gather_gemm: need out [{M}, {N}] and gathered [{M}, {K}], "
+                         f"got {tuple(out.shape)} and {tuple(gathered.shape)}")
+    if _overlap(out, a_shard) or _overlap(gathered, a_shard) or _overlap(out, gathered):
+        raise ValueError("all_gather_gemm: out, gathered and a_shard must not overlap")
+    status_ptr = 0
+    if status is not None:
+        if not (isinstance(status, torch.Tensor) and status.device == device and status.dtype == torch.int32 and
+                status.numel() == 1):
+            raise ValueError("all_gather_gemm: status must be a 1-element int32 tensor on the shard's device")
+        status_ptr = status.data_ptr()
+    _C.all_gather_gemm(accl.impl, accl.wrap_device(a_shard).impl, w.data_ptr(), gathered.data_ptr(), out.data_ptr(),
+                       M, N, K, status_ptr, _stream_handle(accl))
+    return out, gathered
 
 
 def vadd_allreduce(accl: Accl, x: Buffer, y: Buffer, out: Buffer, tmp: Buffer = None, count: int = None,

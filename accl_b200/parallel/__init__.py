@@ -13,6 +13,8 @@ them on a H100 node:
                          (or reduce_scatter + all_gather) per bucket, stream ordered
 * `RowParallelLinear`    TP row-parallel linear whose GEMM epilogue IS the reduce-scatter
                          (wgmma plugin), sequence-parallel output
+* `SeqParallelColumnLinear`  its counterpart: TP column-parallel linear on a sequence-parallel input whose all-gather
+                         feeds the GEMM inside one kernel (wgmma plugin)
 * `ring_exchange`        neighbour send/recv step for context-parallel / ring-attention schedules
 * `process_group`        `torch.distributed` backend "accl" (import accl_b200.parallel.process_group): the standard
                          ProcessGroup interface incl. DistributedDataParallel on top of this library
@@ -306,6 +308,43 @@ class RowParallelLinear(torch.nn.Module):
         out = torch.empty(m // P, self.weight.shape[0], dtype=full.dtype, device=full.device)
         self.group.reduce_scatter_tensor(out, full)
         return out
+
+
+class SeqParallelColumnLinear(torch.nn.Module):
+    """y = all_gather_over_ranks(x_r) @ W_r^T: Megatron column-parallel linear on a sequence-parallel input shard,
+    the counterpart of `RowParallelLinear`.  forward(x_shard [m, in_features]) returns [m * P, out_features_per_rank].
+    On the CUDA backend (bf16, m % 128 == 0, out_features_per_rank % 256 == 0, in_features % 64 == 0) the shard is
+    copied into a heap buffer the layer keeps and one kernel gathers the rows while the GEMM runs
+    (accl_b200.ops.all_gather_gemm); elsewhere falls back to all_gather + matmul.  Every rank must build its layers
+    and run them in the same order (the heap buffer sits at the same offset on every rank)."""
+
+    def __init__(self, group: TensorGroup, in_features, out_features_per_rank, dtype=torch.bfloat16, device=None):
+        super().__init__()
+        self.group = group
+        dev = device if device is not None else (torch.device("cuda", group.accl.cuda_device) if group.accl.is_cuda else "cpu")
+        self.weight = torch.nn.Parameter(torch.empty(out_features_per_rank, in_features, dtype=dtype, device=dev))
+        torch.nn.init.normal_(self.weight, std=0.02)
+        self._shard = None
+
+    @torch.no_grad()
+    def forward(self, x):
+        from ..ops import all_gather_gemm
+        m, k = x.shape
+        P = self.group.world
+        n = self.weight.shape[0]
+        fused_ok = (self.group.accl.is_cuda and self.group.comm_id == 0 and x.dtype == torch.bfloat16 and
+                    self.weight.dtype == torch.bfloat16 and m % 128 == 0 and m * P // 128 <= 1024 and n % 256 == 0 and
+                    k % 64 == 0)
+        if fused_ok:
+            if self._shard is None or self._shard.length != m * k:
+                self._shard = self.group.accl.create_buffer(m * k, torch.bfloat16)
+            shard = self._shard.dev.view(m, k)
+            shard.copy_(x)
+            out, _ = all_gather_gemm(self.group.accl, shard, self.weight.data)
+            return out
+        full = torch.empty(m * P, k, dtype=x.dtype, device=x.device)
+        self.group.all_gather_into_tensor(full, x.contiguous())
+        return full @ self.weight.t()
 
 
 def ring_exchange(group: TensorGroup, send_t: torch.Tensor, recv_t: torch.Tensor, tag=0):

@@ -24,6 +24,7 @@ cudaError_t launch_call(const DevWorld &w, const WorkItem &item, HostCompletion 
 // persistent engine (or a peer rank's spinning kernel on the same GPU).
 void preload_engine_kernels();
 void preload_gemm_rs_kernels();
+void preload_ag_gemm_kernels();
 void preload_vadd_kernels();
 
 // Device-side stream port (the user-kernel <-> engine AXI streams of the reference): a byte

@@ -1,6 +1,6 @@
 // Device-API plugins: compute kernels that talk to the collective machinery
 // themselves (the reference's kernels/plugins/vadd_put pattern, plus the
-// north-star wgmma GEMM whose epilogue feeds a reduce-scatter).
+// north-star wgmma GEMM whose epilogue feeds a reduce-scatter, and the wgmma GEMM fed by an all-gather).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -30,6 +30,23 @@ struct GemmRsArgs {
 // the peer-mapped heap): reduce-scatter along M with no intermediate buffer
 // and no separate collective.  Returns after enqueueing.
 cudaError_t launch_gemm_rs(CudaDevice &dev, const GemmRsArgs &args, cudaStream_t stream);
+
+struct AgGemmArgs {
+  uint64_t a_off;        // heap offset of this rank's [M / P, K] bf16 shard of the activations (the same on every rank)
+  const void *w;         // [N, K] bf16 row-major (this rank's output features, nn.Linear layout)
+  void *gathered;        // [M, K] bf16: receives every rank's shard in rank order
+  void *out;             // [M, N] bf16
+  uint32_t m, n, k;
+  uint32_t *status_dev;  // device word that receives the error bits (0: success) when the kernel ends; may be null
+};
+
+// C = allgather_M(A_shard) * W^T: the first half of a sequence-parallel column-parallel linear layer.  One
+// persistent wgmma kernel computes the tiles of this rank's own rows first while spare warps pull the peers'
+// shards over NVLink into `gathered`, 128 rows at a time and in the order the tiles consume them; a tile of peer rows
+// waits only for its own 128 rows.  Throws std::invalid_argument before enqueueing anything unless
+// M % (128 * P) == 0, N % 256 == 0, K % 64 == 0, M / 128 <= 1024 and every pointer and a_off are 16-byte aligned.
+// Returns after enqueueing.
+cudaError_t launch_ag_gemm(CudaDevice &dev, const AgGemmArgs &args, cudaStream_t stream);
 
 // vector add whose result feeds an all-reduce issued by the kernel itself through the device API (engine must be
 // enabled): out = allreduce_sum(x + y).  The vector is produced in chunks of `chunk_elems` (0: 1 Mi elements); each

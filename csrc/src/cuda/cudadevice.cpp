@@ -256,6 +256,7 @@ CudaDevice::CudaDevice(std::shared_ptr<Oob> oob, const CudaConfig &cfg) : oob_(s
   apply_env_tuning();
   preload_engine_kernels();
   preload_gemm_rs_kernels();
+  preload_ag_gemm_kernels();
   preload_vadd_kernels();
   (void)plugin_scratch(16u << 10); // allocate now: cudaMalloc later could stall behind a running engine kernel
   ACCL_CUDART(launch_reset_ctrl(world_, stream_));

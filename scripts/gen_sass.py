@@ -44,6 +44,16 @@ EXCERPTS = [
      r"UTMAREDG\.2D\.ADD", 30, 6,
      "`UTMAREDG.2D.ADD` = `cp.reduce.async.bulk.tensor.2d ... .add`: the tile is added into "
      "peer memory over NVLink by the TMA unit (device API `reduce_scatter_emit_tile`)."),
+    ("all-gather -> GEMM: MMA issue loop", "k_plugin_ag_gemm", r"HGMMA\.64x256x16", 6, 30,
+     "the same m64n256k16 wgmma mainloop as the single-CTA GEMM -> reduce-scatter, on A tiles of own rows from the local "
+     "shard and of peer rows from `gathered`."),
+    ("all-gather -> GEMM: pull loop over the peer-mapped heap", "k_plugin_ag_gemm", r"LDG\.E\.128\.STRONG\.SYS", 4, 24,
+     "`ld.volatile.global.v4.u32` from the peer's shard through its heap window, four loads in flight per thread before "
+     "their `STG.E.NA.128` stores into the local `gathered` rows."),
+    ("all-gather -> GEMM epilogue: registers -> swizzled smem -> TMA tensor store into C", "k_plugin_ag_gemm",
+     r"UTMASTG\.2D", 30, 6,
+     "`UTMASTG.2D` = `cp.async.bulk.tensor.2d.global.shared::cta.bulk_group`: the bf16 tile leaves shared memory for the "
+     "local C through the TMA unit."),
 ]
 
 
