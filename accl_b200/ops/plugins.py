@@ -17,6 +17,7 @@ import torch
 
 from .. import _C
 from ..core import Accl, Buffer
+from ..utils.dtypes import to_torch
 
 
 def _stream_handle(accl):
@@ -25,32 +26,75 @@ def _stream_handle(accl):
 
 
 def gemm_reduce_scatter(accl: Accl, a: torch.Tensor, w: torch.Tensor, out: Buffer = None, variant: int = 0,
-                        out_dtype=torch.bfloat16) -> Buffer:
+                        out_dtype=None, status: torch.Tensor = None) -> Buffer:
     """out[M/P, N] (in the symmetric heap) = reduce_scatter over ranks of a[M, K_r] @ w[N, K_r]^T.
 
     `a` and `w` are this rank's K-slices (bf16, contiguous, on this rank's GPU).
     Needs M % (128 * world) == 0, N % 256 == 0, K_r % 64 == 0.  Stream ordered.
     The shard is bf16 (partials added in bf16 by the TMA unit) or, with an fp32 `out` buffer / out_dtype, fp32
-    (the P partial products are accumulated without intermediate rounding).  variant: 0 automatic, 1 one CTA per
-    128 x 256 tile, 2 CTA pair (cluster of 2 sharing each W tile) per 256 x 256 tile (needs M % (256 * world) == 0).
+    (the P partial products are accumulated without intermediate rounding); out_dtype defaults to `out`'s dtype, or
+    bf16.  `out` must sit at the same heap offset on every rank: allocate it in the same order everywhere.
+    variant: 0 automatic, 1 one CTA per 128 x 256 tile, 2 CTA pair (cluster of 2 sharing each W tile) per
+    256 x 256 tile (needs M % (256 * world) == 0).
+    `status`, optional 1-element int32 CUDA tensor, receives the error bits when the kernel ends (0: success); with
+    non-zero bits the shard is not a valid result.  A shard at a different heap offset on some peer sets
+    DMA_MISMATCH_ERROR (bit 0) on both ranks, and neither adds into the other's heap.
+    Raises ValueError for a wrong dtype, shape, layout or device, or an `out` that is not a large enough heap buffer.
     """
-    assert a.is_cuda and w.is_cuda and a.dtype == torch.bfloat16 and w.dtype == torch.bfloat16
-    assert a.is_contiguous() and w.is_contiguous() and a.shape[1] == w.shape[1]
+    device = torch.device("cuda", accl.cuda_device)
+    _check_operand("gemm_reduce_scatter", "a", a, device)
+    _check_operand("gemm_reduce_scatter", "w", w, device)
     M, K = a.shape
     N = w.shape[0]
     P = accl.world
+    if w.shape[1] != K:
+        raise ValueError(f"gemm_reduce_scatter: w has K = {w.shape[1]}, a has K = {K}")
+    if M % (128 * P) or N % 256 or K % 64 or not (M and N and K):
+        raise ValueError(f"gemm_reduce_scatter: need M % (128 * {P}) == 0, N % 256 == 0, K % 64 == 0, none of them zero; "
+                         f"got M = {M}, N = {N}, K = {K}")
+    if variant not in (0, 1, 2):
+        raise ValueError(f"gemm_reduce_scatter: variant must be 0, 1 or 2, got {variant}")
+    if variant == 2 and M % (256 * P):
+        raise ValueError(f"gemm_reduce_scatter: the CTA-pair variant needs M % (256 * {P}) == 0, got M = {M}")
+    if out_dtype not in (None, torch.bfloat16, torch.float32):
+        raise ValueError(f"gemm_reduce_scatter: out_dtype must be torch.bfloat16 or torch.float32, got {out_dtype}")
     if out is None:
-        out = accl.create_buffer(M // P * N, out_dtype)
-    assert out.length >= M // P * N
-    _C.gemm_reduce_scatter(accl.impl, a.data_ptr(), w.data_ptr(), out.impl, M, N, K, _stream_handle(accl), variant)
+        out = accl.create_buffer(M // P * N, out_dtype or torch.bfloat16)
+    if not isinstance(out, Buffer) or not accl.heap_contains(_device_view(out)):
+        raise ValueError("gemm_reduce_scatter: out must be a buffer in the symmetric heap (accl.create_buffer)")
+    dt = to_torch(out.dtype)
+    if dt not in (torch.bfloat16, torch.float32) or (out_dtype is not None and dt != out_dtype):
+        raise ValueError(f"gemm_reduce_scatter: out is {dt}; it must be bf16 or fp32"
+                         + (f" and match out_dtype = {out_dtype}" if out_dtype is not None else ""))
+    if out.length < M // P * N:
+        raise ValueError(f"gemm_reduce_scatter: out holds {out.length} elements, the shard needs {M // P * N}")
+    status_ptr = _status_ptr("gemm_reduce_scatter", status, device)
+    _C.gemm_reduce_scatter(accl.impl, a.data_ptr(), w.data_ptr(), out.impl, M, N, K, _stream_handle(accl), variant,
+                           status_ptr)
     return out
 
 
-def _check_operand(name, t, device):
+def _device_view(buf: Buffer):
+    try:
+        return buf.dev
+    except RuntimeError:  # a host-only buffer
+        return None
+
+
+def _check_operand(op, name, t, device):
     if not isinstance(t, torch.Tensor) or t.device != device:
-        raise ValueError(f"all_gather_gemm: {name} must be a tensor on {device}")
+        raise ValueError(f"{op}: {name} must be a tensor on {device}")
     if t.dtype != torch.bfloat16 or t.dim() != 2 or not t.is_contiguous():
-        raise ValueError(f"all_gather_gemm: {name} must be a contiguous 2-D bf16 tensor, got {t.dtype} {tuple(t.shape)}")
+        raise ValueError(f"{op}: {name} must be a contiguous 2-D bf16 tensor, got {t.dtype} {tuple(t.shape)}")
+
+
+def _status_ptr(op, status, device):
+    if status is None:
+        return 0
+    if not (isinstance(status, torch.Tensor) and status.device == device and status.dtype == torch.int32 and
+            status.numel() == 1):
+        raise ValueError(f"{op}: status must be a 1-element int32 tensor on {device}")
+    return status.data_ptr()
 
 
 def _overlap(a: torch.Tensor, b: torch.Tensor) -> bool:
@@ -75,8 +119,8 @@ def all_gather_gemm(accl: Accl, a_shard: torch.Tensor, w: torch.Tensor, out: tor
     if not isinstance(a_shard, torch.Tensor) or not accl.heap_contains(a_shard):
         raise ValueError("all_gather_gemm: a_shard must live in the symmetric heap (a Buffer.dev view or a heap_mem_pool tensor)")
     device = a_shard.device
-    _check_operand("a_shard", a_shard, device)
-    _check_operand("w", w, device)
+    _check_operand("all_gather_gemm", "a_shard", a_shard, device)
+    _check_operand("all_gather_gemm", "w", w, device)
     m, K = a_shard.shape
     M, N = m * accl.world, w.shape[0]
     if w.shape[1] != K:
@@ -85,19 +129,14 @@ def all_gather_gemm(accl: Accl, a_shard: torch.Tensor, w: torch.Tensor, out: tor
         out = torch.empty(M, N, dtype=torch.bfloat16, device=device)
     if gathered is None:
         gathered = torch.empty(M, K, dtype=torch.bfloat16, device=device)
-    _check_operand("out", out, device)
-    _check_operand("gathered", gathered, device)
+    _check_operand("all_gather_gemm", "out", out, device)
+    _check_operand("all_gather_gemm", "gathered", gathered, device)
     if tuple(out.shape) != (M, N) or tuple(gathered.shape) != (M, K):
         raise ValueError(f"all_gather_gemm: need out [{M}, {N}] and gathered [{M}, {K}], "
                          f"got {tuple(out.shape)} and {tuple(gathered.shape)}")
     if _overlap(out, a_shard) or _overlap(gathered, a_shard) or _overlap(out, gathered):
         raise ValueError("all_gather_gemm: out, gathered and a_shard must not overlap")
-    status_ptr = 0
-    if status is not None:
-        if not (isinstance(status, torch.Tensor) and status.device == device and status.dtype == torch.int32 and
-                status.numel() == 1):
-            raise ValueError("all_gather_gemm: status must be a 1-element int32 tensor on the shard's device")
-        status_ptr = status.data_ptr()
+    status_ptr = _status_ptr("all_gather_gemm", status, device)
     _C.all_gather_gemm(accl.impl, accl.wrap_device(a_shard).impl, w.data_ptr(), gathered.data_ptr(), out.data_ptr(),
                        M, N, K, status_ptr, _stream_handle(accl))
     return out, gathered

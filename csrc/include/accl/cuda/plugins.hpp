@@ -21,6 +21,7 @@ struct GemmRsArgs {
   uint32_t epoch;    // launch counter (same on every rank), starts at 1
   int variant = 0;   // 0: automatic, 1: one CTA per 128 x 256 tile, 2: CTA pair (cluster of 2, W tile multicast) per 256 x 256 tile
   bool out_f32 = false; // shard is fp32: the P partial products are added without intermediate rounding
+  uint32_t *status_dev = nullptr; // device word that receives the error bits (0: success) when the kernel ends; may be null
 };
 
 // C = A * W^T computed tile by tile on the tensor cores (TMA -> smem ->
@@ -28,7 +29,9 @@ struct GemmRsArgs {
 // to bf16, staged in shared memory and added straight into its owner rank's
 // output shard over NVLink by the TMA unit (cp.reduce.async.bulk.tensor .add on
 // the peer-mapped heap): reduce-scatter along M with no intermediate buffer
-// and no separate collective.  Returns after enqueueing.
+// and no separate collective.  The shard must sit at out_off on every rank: no tile is added into a peer whose
+// shard is elsewhere, and the call reports DMA_MISMATCH_ERROR.  With non-zero status bits the shard is not a valid
+// result.  Returns after enqueueing.
 cudaError_t launch_gemm_rs(CudaDevice &dev, const GemmRsArgs &args, cudaStream_t stream);
 
 struct AgGemmArgs {

@@ -132,17 +132,18 @@ void bind_cuda(py::module_ &m) {
   });
   // out_shard[M/P, N] (heap buffer, bf16) = reduce_scatter_M( A[M,K] @ W[N,K]^T ), fused on wgmma + NVLink
   m.def("gemm_reduce_scatter", [](ACCL &a, uintptr_t a_ptr, uintptr_t w_ptr, BaseBuffer &out, uint32_t M, uint32_t N, uint32_t K,
-                                  uintptr_t stream, int variant) {
+                                  uintptr_t stream, int variant, uintptr_t status_dev_ptr) {
     auto *d = dynamic_cast<CudaDevice *>(a.device());
     if (!d) throw std::runtime_error("not a CUDA backend");
     GemmRsArgs g{reinterpret_cast<const void *>(a_ptr), reinterpret_cast<const void *>(w_ptr), out.address(), M, N, K, 0};
     g.variant = variant;
     g.out_f32 = out.type() == dataType::float32;
+    g.status_dev = reinterpret_cast<uint32_t *>(status_dev_ptr);
     if (!g.out_f32 && out.type() != dataType::bfloat16) throw std::invalid_argument("gemm_reduce_scatter: output shard must be bf16 or fp32");
     cudaError_t e = launch_gemm_rs(*d, g, reinterpret_cast<cudaStream_t>(stream));
     if (e != cudaSuccess) throw std::runtime_error(std::string("gemm_reduce_scatter launch: ") + cudaGetErrorString(e));
   }, py::arg("accl"), py::arg("a_ptr"), py::arg("w_ptr"), py::arg("out"), py::arg("M"), py::arg("N"), py::arg("K"), py::arg("stream"),
-        py::arg("variant") = 0, py::call_guard<py::gil_scoped_release>());
+        py::arg("variant") = 0, py::arg("status_dev_ptr") = 0, py::call_guard<py::gil_scoped_release>());
   // out[M, N] = allgather_M(shard[M/P, K]) @ W[N, K]^T, fused on wgmma + NVLink; gathered[M, K] receives the gathered rows
   m.def("all_gather_gemm", [](ACCL &a, BaseBuffer &shard, uintptr_t w_ptr, uintptr_t gathered_ptr, uintptr_t out_ptr, uint32_t M,
                               uint32_t N, uint32_t K, uintptr_t status_dev_ptr, uintptr_t stream) {

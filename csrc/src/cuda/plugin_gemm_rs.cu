@@ -94,6 +94,7 @@ struct GemmRsParams {
   uint32_t epoch;
   uint32_t timeout_us;
   unsigned int *grid_flags; // zeroed before every launch: [0] zero-phase arrivals, [1] release, [2] finished CTAs, [3] error, [8..] peer offsets
+  uint32_t *status;         // receives the error bits (0: success) when the kernel ends; may be null
 };
 
 
@@ -188,13 +189,20 @@ k_plugin_gemm_rs(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         while (atomicAdd(&p.grid_flags[0], 0u) < gridDim.x) dev::nanosleep(100);
       __syncwarp();
       __threadfence();
+      // the output tensor maps assume the shard sits at out_off in every heap: a peer that does not answer, is in
+      // another operation or has its shard elsewhere gets no reduce-adds (INVALID_OFF, or its differing offset)
       uint64_t peer_off = p.out_off;
       if (static_cast<uint32_t>(lane) < P && static_cast<uint32_t>(lane) != me) {
         k::pad_post(ctx, MAX_CH - 1, lane, k::REC_OFFS, p.out_off, p.out_off, ctx.kind_word());
+        peer_off = INVALID_OFF;
         if (k::pad_wait(ctx, MAX_CH - 1, lane)) {
           const SyncRec r = k::pad_rec(ctx, MAX_CH - 1, lane, k::REC_OFF0);
-          peer_off = r.off0;
-          if (r.kind != ctx.kind_word()) atomicOr(&s_err, PACK_SEQ_NUMBER_ERROR);
+          if (r.kind != ctx.kind_word()) {
+            atomicOr(&s_err, PACK_SEQ_NUMBER_ERROR);
+          } else {
+            peer_off = r.off0;
+            if (peer_off != p.out_off) atomicOr(&s_err, DMA_MISMATCH_ERROR);
+          }
         }
       }
       if (static_cast<uint32_t>(lane) < P) reinterpret_cast<volatile uint64_t *>(p.grid_flags + 8)[lane] = peer_off;
@@ -238,7 +246,7 @@ k_plugin_gemm_rs(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     const bool signaller = threadIdx.x % 128 == 0;
     uint8_t *my_epi = smem_epi + (warp - 4) * 2 * EPI_BUF_BYTES;
     uint32_t stage = 0, phase = 0, ebuf = 0;
-    bool released = false;
+    uint32_t owners_ok = 0; // owners whose shard sits at out_off, the only ones this warp adds into; 0: not yet released
     float d[128];
 #pragma unroll
     for (int i = 0; i < 128; ++i) d[i] = 0.f;
@@ -273,7 +281,7 @@ k_plugin_gemm_rs(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       wgmma_wait<0>();
       release(prev);
 
-      if (!released) {
+      if (!owners_ok) {
         if (lane == 0) {
           uint32_t spins = 0;
           while (*reinterpret_cast<volatile unsigned int *>(&p.grid_flags[1]) == 0)
@@ -283,15 +291,13 @@ k_plugin_gemm_rs(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         __threadfence();
         // every shard has been zeroed with generic stores: order them before this warp's TMA reduce-adds
         asm volatile("fence.proxy.async.global;" ::: "memory");
-        // shards must sit at the same heap offset on every rank (the output tensor maps assume it)
-        if (static_cast<uint32_t>(lane) < P && reinterpret_cast<const volatile uint64_t *>(p.grid_flags + 8)[lane] != p.out_off)
-          atomicOr(&p.grid_flags[3], static_cast<unsigned>(DMA_MISMATCH_ERROR));
-        released = true;
+        owners_ok = (1u << me) | __ballot_sync(0xffffffffu, static_cast<uint32_t>(lane) < P &&
+                                                              reinterpret_cast<const volatile uint64_t *>(p.grid_flags + 8)[lane] == p.out_off);
       }
       const uint32_t row0 = mb * C::TILE_M + cr * BM + wg * 64 + wi * EPI_ROWS; // first of this warp's 16 rows
       const uint32_t owner = row0 / rows_per_rank;                              // a warp's rows never straddle owners
       const int local_row0 = static_cast<int>(row0 - owner * rows_per_rank);
-      emit_chunks<F32, 0>(d, my_epi, ebuf, lane, &out_maps.m[owner], static_cast<int>(nb * BN), local_row0);
+      if ((owners_ok >> owner) & 1u) emit_chunks<F32, 0>(d, my_epi, ebuf, lane, &out_maps.m[owner], static_cast<int>(nb * BN), local_row0);
     }
     if (lane == 0) device::emit_flush(); // all my reductions have completed
     __syncwarp();
@@ -303,6 +309,7 @@ k_plugin_gemm_rs(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   if (PAIR) cluster_sync(); // nobody exits while the peer may still signal its barriers or write its smem
   __shared__ uint32_t s_last;
   if (threadIdx.x == 0) {
+    if (s_err) atomicOr(&p.grid_flags[3], s_err);
     __threadfence_system();
     s_last = atomicAdd(&p.grid_flags[2], 1u) == gridDim.x - 1 ? 1u : 0u;
   }
@@ -310,7 +317,7 @@ k_plugin_gemm_rs(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   if (s_last) {
     // every CTA of this rank has pushed its tiles: when all ranks meet here, every shard is complete
     k::chan_sync(ctx, false, 0, 0, nullptr, nullptr);
-    if (threadIdx.x == 0 && s_err) atomicOr(&p.grid_flags[3], s_err);
+    if (threadIdx.x == 0 && p.status) *p.status = atomicOr(&p.grid_flags[3], s_err) | s_err;
   }
 }
 
@@ -399,7 +406,8 @@ cudaError_t launch_gemm_rs(CudaDevice &dev, const GemmRsArgs &a, cudaStream_t st
   const CUtensorMap tb = make_map(a.w, a.n, a.k, pair ? BN / 2 : BN, BK); // each CTA of a pair loads half of the N tile
   OutMaps om;
   std::memset(&om, 0, sizeof(om));
-  for (uint32_t o = 0; o < P; ++o) // symmetric allocation: the shard sits at out_off in every heap (verified in-kernel)
+  for (uint32_t o = 0; o < P; ++o) // symmetric allocation: the shard sits at out_off in every heap (verified in-kernel:
+                                   // an owner whose shard is elsewhere gets no adds and the call reports DMA_MISMATCH_ERROR)
     om.m[o] = make_map(dev.world().window + static_cast<uint64_t>(o) * dev.world().heap_bytes + a.out_off, a.m / P, a.n, EPI_ROWS,
                        f32 ? 32 : 64, f32);
   GemmRsParams p;
@@ -411,6 +419,7 @@ cudaError_t launch_gemm_rs(CudaDevice &dev, const GemmRsArgs &a, cudaStream_t st
   p.epoch = a.epoch;
   p.timeout_us = dev.timeout_us();
   p.grid_flags = st->flags;
+  p.status = a.status_dev;
   int sms = 0;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev.device());
   ACCL_CUDART(cudaMemsetAsync(st->flags, 0, 64 * sizeof(unsigned int), stream));
