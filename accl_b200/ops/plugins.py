@@ -26,10 +26,12 @@ def _stream_handle(accl):
 
 
 def gemm_reduce_scatter(accl: Accl, a: torch.Tensor, w: torch.Tensor, out: Buffer = None, variant: int = 0,
-                        out_dtype=None, status: torch.Tensor = None) -> Buffer:
+                        out_dtype=None, status: torch.Tensor = None, w_layout: str = "nk") -> Buffer:
     """out[M/P, N] (in the symmetric heap) = reduce_scatter over ranks of a[M, K_r] @ w[N, K_r]^T.
 
-    `a` and `w` are this rank's K-slices (bf16, contiguous, on this rank's GPU).
+    `a` and `w` are this rank's K-slices (bf16, contiguous, on this rank's GPU).  w_layout "nk" (default): `w` is
+    [N, K_r] (nn.Linear layout); "kn": `w` is [K_r, N] and the product is a @ w, e.g. an nn.Linear weight in its own
+    backward pass, dX = reduce_scatter(dY @ W), without a transposed copy.
     Needs M % (128 * world) == 0, N % 256 == 0, K_r % 64 == 0.  Stream ordered.
     The shard is bf16 (partials added in bf16 by the TMA unit) or, with an fp32 `out` buffer / out_dtype, fp32
     (the P partial products are accumulated without intermediate rounding); out_dtype defaults to `out`'s dtype, or
@@ -44,11 +46,12 @@ def gemm_reduce_scatter(accl: Accl, a: torch.Tensor, w: torch.Tensor, out: Buffe
     device = torch.device("cuda", accl.cuda_device)
     _check_operand("gemm_reduce_scatter", "a", a, device)
     _check_operand("gemm_reduce_scatter", "w", w, device)
+    kn = _is_kn("gemm_reduce_scatter", w_layout)
     M, K = a.shape
-    N = w.shape[0]
+    N, w_k = (w.shape[1], w.shape[0]) if kn else (w.shape[0], w.shape[1])
     P = accl.world
-    if w.shape[1] != K:
-        raise ValueError(f"gemm_reduce_scatter: w has K = {w.shape[1]}, a has K = {K}")
+    if w_k != K:
+        raise ValueError(f"gemm_reduce_scatter: w has K = {w_k}, a has K = {K}")
     if M % (128 * P) or N % 256 or K % 64 or not (M and N and K):
         raise ValueError(f"gemm_reduce_scatter: need M % (128 * {P}) == 0, N % 256 == 0, K % 64 == 0, none of them zero; "
                          f"got M = {M}, N = {N}, K = {K}")
@@ -70,8 +73,14 @@ def gemm_reduce_scatter(accl: Accl, a: torch.Tensor, w: torch.Tensor, out: Buffe
         raise ValueError(f"gemm_reduce_scatter: out holds {out.length} elements, the shard needs {M // P * N}")
     status_ptr = _status_ptr("gemm_reduce_scatter", status, device)
     _C.gemm_reduce_scatter(accl.impl, a.data_ptr(), w.data_ptr(), out.impl, M, N, K, _stream_handle(accl), variant,
-                           status_ptr)
+                           status_ptr, kn)
     return out
+
+
+def _is_kn(op, w_layout):
+    if w_layout not in ("nk", "kn"):
+        raise ValueError(f'{op}: w_layout must be "nk" or "kn", got {w_layout!r}')
+    return w_layout == "kn"
 
 
 def _device_view(buf: Buffer):
@@ -103,12 +112,13 @@ def _overlap(a: torch.Tensor, b: torch.Tensor) -> bool:
 
 
 def all_gather_gemm(accl: Accl, a_shard: torch.Tensor, w: torch.Tensor, out: torch.Tensor = None,
-                    gathered: torch.Tensor = None, status: torch.Tensor = None):
+                    gathered: torch.Tensor = None, status: torch.Tensor = None, w_layout: str = "nk"):
     """out[M, N] = all_gather over ranks of a_shard[M/P, K], times w[N, K]^T.  Returns (out, gathered).
 
     `a_shard` is this rank's rows, a contiguous bf16 tensor in the symmetric heap (a `Buffer.dev` view or a tensor
     from `heap_mem_pool()`), at the same heap offset on every rank: allocate it in the same order everywhere.
-    `w` is this rank's output features (bf16, nn.Linear layout).  `out` (bf16 [M, N]) and `gathered` (bf16 [M, K],
+    `w` is this rank's output features (bf16, nn.Linear layout); with w_layout "kn" it is [K, N] and the product is
+    gathered @ w, e.g. an nn.Linear weight in its own backward pass, dX = all_gather(dY) @ W.  `out` (bf16 [M, N]) and `gathered` (bf16 [M, K],
     every rank's shard in rank order) are ordinary CUDA tensors, allocated when not given.  Needs M % (128 * P) == 0,
     N % 256 == 0, K % 64 == 0 and M <= 128 * 1024.  Stream ordered: a rank may rewrite its shard on the stream right
     after the call.
@@ -121,10 +131,12 @@ def all_gather_gemm(accl: Accl, a_shard: torch.Tensor, w: torch.Tensor, out: tor
     device = a_shard.device
     _check_operand("all_gather_gemm", "a_shard", a_shard, device)
     _check_operand("all_gather_gemm", "w", w, device)
+    kn = _is_kn("all_gather_gemm", w_layout)
     m, K = a_shard.shape
-    M, N = m * accl.world, w.shape[0]
-    if w.shape[1] != K:
-        raise ValueError(f"all_gather_gemm: w has K = {w.shape[1]}, a_shard has K = {K}")
+    M, N = m * accl.world, (w.shape[1] if kn else w.shape[0])
+    w_k = w.shape[0] if kn else w.shape[1]
+    if w_k != K:
+        raise ValueError(f"all_gather_gemm: w has K = {w_k}, a_shard has K = {K}")
     if out is None:
         out = torch.empty(M, N, dtype=torch.bfloat16, device=device)
     if gathered is None:
@@ -138,7 +150,7 @@ def all_gather_gemm(accl: Accl, a_shard: torch.Tensor, w: torch.Tensor, out: tor
         raise ValueError("all_gather_gemm: out, gathered and a_shard must not overlap")
     status_ptr = _status_ptr("all_gather_gemm", status, device)
     _C.all_gather_gemm(accl.impl, accl.wrap_device(a_shard).impl, w.data_ptr(), gathered.data_ptr(), out.data_ptr(),
-                       M, N, K, status_ptr, _stream_handle(accl))
+                       M, N, K, status_ptr, _stream_handle(accl), kn)
     return out, gathered
 
 

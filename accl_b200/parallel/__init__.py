@@ -12,9 +12,10 @@ them on a H100 node:
 * `GradBucket`           DP / ZeRO gradient bucket living in the heap: fill, then one all-reduce
                          (or reduce_scatter + all_gather) per bucket, stream ordered
 * `RowParallelLinear`    TP row-parallel linear whose GEMM epilogue IS the reduce-scatter
-                         (wgmma plugin), sequence-parallel output
+                         (wgmma plugin), sequence-parallel output; its input gradient runs on the all-gather plugin
 * `SeqParallelColumnLinear`  its counterpart: TP column-parallel linear on a sequence-parallel input whose all-gather
-                         feeds the GEMM inside one kernel (wgmma plugin)
+                         feeds the GEMM inside one kernel (wgmma plugin); its input gradient runs on the
+                         reduce-scatter plugin
 * `ring_exchange`        neighbour send/recv step for context-parallel / ring-attention schedules
 * `process_group`        `torch.distributed` backend "accl" (import accl_b200.parallel.process_group): the standard
                          ProcessGroup interface incl. DistributedDataParallel on top of this library
@@ -79,6 +80,7 @@ class TensorGroup:
         # its side), so a staged receive has to be waited for on the host before its staging buffer is read
         self._engine = bool(accl.is_cuda) and "mode=engine" in accl.describe()
         self._pending = []  # asynchronous requests whose return code has not been looked at yet
+        self._plugin_status = None  # int32 device word: OR of the status bits of every fused plugin call (CUDA)
 
     # -- request bookkeeping ---------------------------------------------------
     def _track(self, req):
@@ -90,8 +92,27 @@ class TensorGroup:
         self.check(block=len(self._pending) > 64)
         return req
 
+    def plugin_status(self):
+        """A fresh 1-element int32 status tensor for one fused plugin call (ops.gemm_reduce_scatter /
+        ops.all_gather_gemm); pass it to the call, then to `note_plugin_status`."""
+        return torch.zeros(1, dtype=torch.int32, device=torch.device("cuda", self.accl.cuda_device))
+
+    def note_plugin_status(self, status):
+        """OR a fused call's status word into this group's, stream ordered: nothing waits for the host, so it may run
+        inside autograd's backward.  `check(block=True)` and `barrier()` raise when the word is non-zero."""
+        if self._plugin_status is None:
+            self._plugin_status = torch.zeros_like(status)
+        self._plugin_status.bitwise_or_(status)
+
     def check(self, block=False):
-        """Raise if any finished call reported an error; with block=True wait for everything outstanding."""
+        """Raise if any finished call reported an error; with block=True wait for everything outstanding, including the
+        fused plugin calls of this group's layers (their status word is read then, and cleared)."""
+        if block and self._plugin_status is not None:
+            bits = int(self._plugin_status.item())
+            if bits:
+                self._plugin_status.zero_()
+                raise RuntimeError(f"fused GEMM plugin call failed on rank {self.rank}: {_C.error_to_string(bits)} "
+                                   f"(0x{bits:x})")
         keep = []
         for r in self._pending:
             if block:
@@ -279,10 +300,134 @@ class GradBucket:
         return out
 
 
+def row_forward_fused(cuda, dtype, m, world, out_features, in_features_per_rank):
+    """Whether RowParallelLinear's forward runs on ops.gemm_reduce_scatter: [m, K_r] @ [N, K_r]^T, reduce-scattered."""
+    return (cuda and dtype == torch.bfloat16 and m % (128 * world) == 0 and out_features % 256 == 0 and
+            in_features_per_rank % 64 == 0)
+
+
+def row_backward_fused(cuda, comm_id, dtype, m, world, out_features, in_features_per_rank):
+    """Whether RowParallelLinear's input gradient runs on ops.all_gather_gemm: dX_r = all_gather(dY_shard) @ W_r, the
+    weight [N, K_r] read as [K, N] ("kn"): output columns K_r % 256, contraction N % 64."""
+    return (cuda and comm_id == 0 and dtype == torch.bfloat16 and m % (128 * world) == 0 and m // 128 <= 1024 and
+            in_features_per_rank % 256 == 0 and out_features % 64 == 0)
+
+
+def column_forward_fused(cuda, comm_id, dtype, m, world, in_features, out_features_per_rank):
+    """Whether SeqParallelColumnLinear's forward runs on ops.all_gather_gemm: all_gather(x [m, K]) @ [N_r, K]^T."""
+    return (cuda and comm_id == 0 and dtype == torch.bfloat16 and m % 128 == 0 and m * world // 128 <= 1024 and
+            out_features_per_rank % 256 == 0 and in_features % 64 == 0)
+
+
+def column_backward_fused(cuda, comm_id, dtype, m, world, in_features, out_features_per_rank):
+    """Whether SeqParallelColumnLinear's input gradient runs on ops.gemm_reduce_scatter: dX_shard =
+    reduce_scatter(dY [m P, N_r] @ W), the weight [N_r, K] read as [K, N] ("kn"): output columns K % 256, contraction
+    N_r % 64."""
+    return (cuda and comm_id == 0 and dtype == torch.bfloat16 and m % 128 == 0 and in_features % 256 == 0 and
+            out_features_per_rank % 64 == 0)
+
+
+def _heap_buffer(layer, attr, n):
+    """The layer's heap buffer `attr` of n bf16 elements, (re)allocated here: in forward, in the rank's own thread and
+    in layer order, so it sits at the same heap offset on every rank."""
+    buf = getattr(layer, attr)
+    if buf is None or buf.length != n:
+        buf = layer.group.accl.create_buffer(n, torch.bfloat16)
+        setattr(layer, attr, buf)
+    return buf
+
+
+def _dtype_of(x, weight):
+    return x.dtype if x.dtype == weight.dtype else None
+
+
+def _wants_grad(x, weight):
+    return torch.is_grad_enabled() and (x.requires_grad or weight.requires_grad)
+
+
+class _RowParallelFn(torch.autograd.Function):
+    """y_shard = reduce_scatter(x_r W_r^T); dX_r = all_gather(dY_shard) W_r, dW_r = all_gather(dY_shard)^T x_r."""
+
+    @staticmethod
+    def forward(ctx, x, weight, layer):
+        group = layer.group
+        m, k = x.shape
+        n, P = weight.shape[0], group.world
+        cuda = bool(group.accl.is_cuda)
+        ctx.layer, ctx.m = layer, m
+        ctx.bwd_fused = row_backward_fused(cuda, group.comm_id, _dtype_of(x, weight), m, P, n, k)
+        ctx.dy_buf = _heap_buffer(layer, "_dy_shard", m // P * n) if ctx.bwd_fused else None
+        ctx.save_for_backward(x, weight)
+        return layer._forward(x, weight, training=True)
+
+    @staticmethod
+    def backward(ctx, dy):
+        from ..ops import all_gather_gemm
+        x, weight = ctx.saved_tensors
+        group = ctx.layer.group
+        dy = dy.contiguous()
+        dx = None
+        if ctx.bwd_fused:
+            shard = ctx.dy_buf.dev.view(dy.shape)
+            shard.copy_(dy)
+            st = group.plugin_status()
+            dx, gathered = all_gather_gemm(group.accl, shard, weight.detach(), status=st, w_layout="kn")
+            group.note_plugin_status(st)
+        else:
+            gathered = torch.empty(ctx.m, dy.shape[1], dtype=dy.dtype, device=dy.device)
+            group.all_gather_into_tensor(gathered, dy)
+            if ctx.needs_input_grad[0]:
+                dx = gathered @ weight
+        dw = gathered.t() @ x if ctx.needs_input_grad[1] else None
+        return (dx if ctx.needs_input_grad[0] else None), dw, None
+
+
+class _ColumnParallelFn(torch.autograd.Function):
+    """y = all_gather(x_r) W_r^T; dX_r = reduce_scatter(dY W_r), dW_r = dY^T all_gather(x_r)."""
+
+    @staticmethod
+    def forward(ctx, x, weight, layer):
+        group = layer.group
+        m, k = x.shape
+        n, P = weight.shape[0], group.world
+        cuda = bool(group.accl.is_cuda)
+        ctx.layer, ctx.m = layer, m
+        ctx.bwd_fused = column_backward_fused(cuda, group.comm_id, _dtype_of(x, weight), m, P, k, n)
+        ctx.dx_buf = _heap_buffer(layer, "_dx_shard", m * k) if ctx.bwd_fused and ctx.needs_input_grad[0] else None
+        out, gathered = layer._forward(x, weight, training=True)
+        ctx.save_for_backward(gathered, weight)
+        return out
+
+    @staticmethod
+    def backward(ctx, dy):
+        from ..ops import gemm_reduce_scatter
+        gathered, weight = ctx.saved_tensors
+        group = ctx.layer.group
+        dy = dy.contiguous()
+        dx = None
+        if ctx.needs_input_grad[0]:
+            if ctx.bwd_fused:
+                st = group.plugin_status()
+                gemm_reduce_scatter(group.accl, dy, weight.detach(), ctx.dx_buf, status=st, w_layout="kn")
+                group.note_plugin_status(st)
+                # the heap buffer is rewritten by the next backward through this layer
+                dx = ctx.dx_buf.dev.view(ctx.m, weight.shape[1]).clone()
+            else:
+                dx = torch.empty(ctx.m, weight.shape[1], dtype=dy.dtype, device=dy.device)
+                group.reduce_scatter_tensor(dx, (dy @ weight).contiguous())
+        dw = dy.t() @ gathered if ctx.needs_input_grad[1] else None
+        return dx, dw, None
+
+
 class RowParallelLinear(torch.nn.Module):
     """y = reduce_scatter_over_ranks(x_r @ W_r^T): Megatron row-parallel linear with a sequence-parallel
     output shard.  On the CUDA backend the GEMM (wgmma) emits its tiles straight into the owner rank's
-    shard over NVLink (accl_b200.ops.gemm_reduce_scatter); elsewhere falls back to matmul + reduce_scatter."""
+    shard over NVLink (accl_b200.ops.gemm_reduce_scatter); elsewhere falls back to matmul + reduce_scatter.
+    Trainable: with grad enabled the input gradient dX_r = all_gather(dY_shard) @ W_r runs on
+    accl_b200.ops.all_gather_gemm reading W_r as [K, N] (no transposed copy) when the shape allows it
+    (`row_backward_fused`), else on all_gather + matmul; dW_r = all_gather(dY_shard)^T @ x_r is a local matmul.
+    Every rank must build its layers and run them in the same order (the heap buffers sit at the same offset on every
+    rank), and fused-call errors surface at `group.check(block=True)` / `group.barrier()`."""
 
     def __init__(self, group: TensorGroup, in_features_per_rank, out_features, dtype=torch.bfloat16, device=None):
         super().__init__()
@@ -291,21 +436,32 @@ class RowParallelLinear(torch.nn.Module):
         self.weight = torch.nn.Parameter(torch.empty(out_features, in_features_per_rank, dtype=dtype, device=dev))
         torch.nn.init.normal_(self.weight, std=0.02)
         self._out = None
+        self._dy_shard = None  # heap buffer of the fused backward's all-gather operand
 
-    @torch.no_grad()
     def forward(self, x):
+        if _wants_grad(x, self.weight):
+            return _RowParallelFn.apply(x, self.weight, self)
+        with torch.no_grad():
+            return self._forward(x, self.weight)
+
+    def _forward(self, x, weight, training=False):
+        """training: the fused call reports into the group's status word, and the result is copied out of the layer's
+        heap buffer, which the next call rewrites (micro-batches, recomputation)."""
         from ..ops import gemm_reduce_scatter
         m = x.shape[0]
         P = self.group.world
-        fused_ok = (self.group.accl.is_cuda and x.dtype == torch.bfloat16 and m % (128 * P) == 0 and
-                    self.weight.shape[0] % 256 == 0 and self.weight.shape[1] % 64 == 0)
-        if fused_ok:
-            if self._out is None or self._out.length != m // P * self.weight.shape[0]:
-                self._out = self.group.accl.create_buffer(m // P * self.weight.shape[0], torch.bfloat16)
-            gemm_reduce_scatter(self.group.accl, x.contiguous(), self.weight.data, self._out)
-            return self._out.dev.view(m // P, self.weight.shape[0])
-        full = x @ self.weight.t()
-        out = torch.empty(m // P, self.weight.shape[0], dtype=full.dtype, device=full.device)
+        if row_forward_fused(bool(self.group.accl.is_cuda), x.dtype, m, P, weight.shape[0], weight.shape[1]):
+            if self._out is None or self._out.length != m // P * weight.shape[0]:
+                self._out = self.group.accl.create_buffer(m // P * weight.shape[0], torch.bfloat16)
+            if training:
+                st = self.group.plugin_status()
+                gemm_reduce_scatter(self.group.accl, x.contiguous(), weight.detach(), self._out, status=st)
+                self.group.note_plugin_status(st)
+                return self._out.dev.view(m // P, weight.shape[0]).clone()
+            gemm_reduce_scatter(self.group.accl, x.contiguous(), weight.data, self._out)
+            return self._out.dev.view(m // P, weight.shape[0])
+        full = x @ weight.t()
+        out = torch.empty(m // P, weight.shape[0], dtype=full.dtype, device=full.device)
         self.group.reduce_scatter_tensor(out, full)
         return out
 
@@ -316,7 +472,11 @@ class SeqParallelColumnLinear(torch.nn.Module):
     On the CUDA backend (bf16, m % 128 == 0, out_features_per_rank % 256 == 0, in_features % 64 == 0) the shard is
     copied into a heap buffer the layer keeps and one kernel gathers the rows while the GEMM runs
     (accl_b200.ops.all_gather_gemm); elsewhere falls back to all_gather + matmul.  Every rank must build its layers
-    and run them in the same order (the heap buffer sits at the same offset on every rank)."""
+    and run them in the same order (the heap buffer sits at the same offset on every rank).
+    Trainable: with grad enabled the input gradient dX_shard = reduce_scatter(dY @ W_r) runs on
+    accl_b200.ops.gemm_reduce_scatter reading W_r as [K, N] (no transposed copy) when the shape allows it
+    (`column_backward_fused`), else on matmul + reduce_scatter; dW_r = dY^T @ gathered reuses the gathered input the
+    forward returns.  Fused-call errors surface at `group.check(block=True)` / `group.barrier()`."""
 
     def __init__(self, group: TensorGroup, in_features, out_features_per_rank, dtype=torch.bfloat16, device=None):
         super().__init__()
@@ -325,26 +485,34 @@ class SeqParallelColumnLinear(torch.nn.Module):
         self.weight = torch.nn.Parameter(torch.empty(out_features_per_rank, in_features, dtype=dtype, device=dev))
         torch.nn.init.normal_(self.weight, std=0.02)
         self._shard = None
+        self._dx_shard = None  # heap buffer of the fused backward's reduce-scattered input gradient
 
-    @torch.no_grad()
     def forward(self, x):
+        if _wants_grad(x, self.weight):
+            return _ColumnParallelFn.apply(x, self.weight, self)
+        with torch.no_grad():
+            return self._forward(x, self.weight)[0]
+
+    def _forward(self, x, weight, training=False):
+        """(y, the gathered input [m P, in_features]); training: the fused call reports into the group's status word."""
         from ..ops import all_gather_gemm
         m, k = x.shape
         P = self.group.world
-        n = self.weight.shape[0]
-        fused_ok = (self.group.accl.is_cuda and self.group.comm_id == 0 and x.dtype == torch.bfloat16 and
-                    self.weight.dtype == torch.bfloat16 and m % 128 == 0 and m * P // 128 <= 1024 and n % 256 == 0 and
-                    k % 64 == 0)
-        if fused_ok:
+        n = weight.shape[0]
+        if column_forward_fused(bool(self.group.accl.is_cuda), self.group.comm_id, _dtype_of(x, weight), m, P, k, n):
             if self._shard is None or self._shard.length != m * k:
                 self._shard = self.group.accl.create_buffer(m * k, torch.bfloat16)
             shard = self._shard.dev.view(m, k)
             shard.copy_(x)
-            out, _ = all_gather_gemm(self.group.accl, shard, self.weight.data)
-            return out
+            if training:
+                st = self.group.plugin_status()
+                out, gathered = all_gather_gemm(self.group.accl, shard, weight.detach(), status=st)
+                self.group.note_plugin_status(st)
+                return out, gathered
+            return all_gather_gemm(self.group.accl, shard, weight.data)
         full = torch.empty(m * P, k, dtype=x.dtype, device=x.device)
         self.group.all_gather_into_tensor(full, x.contiguous())
-        return full @ self.weight.t()
+        return full @ weight.t(), full
 
 
 def ring_exchange(group: TensorGroup, send_t: torch.Tensor, recv_t: torch.Tensor, tag=0):

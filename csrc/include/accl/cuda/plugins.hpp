@@ -15,16 +15,17 @@ class CudaDevice;
 
 struct GemmRsArgs {
   const void *a;     // [M, K] bf16 row-major (this rank's K-slice of the activations)
-  const void *w;     // [N, K] bf16 row-major (this rank's K-slice of the weight, nn.Linear layout)
+  const void *w;     // [N, K] bf16 row-major (this rank's K-slice of the weight, nn.Linear layout), or [K, N] with w_kn
   uint64_t out_off;  // heap offset of this rank's [M / P, N] output shard (bf16, or fp32 with out_f32)
   uint32_t m, n, k;
   uint32_t epoch;    // launch counter (same on every rank), starts at 1
   int variant = 0;   // 0: automatic, 1: one CTA per 128 x 256 tile, 2: CTA pair (cluster of 2, W tile multicast) per 256 x 256 tile
   bool out_f32 = false; // shard is fp32: the P partial products are added without intermediate rounding
   uint32_t *status_dev = nullptr; // device word that receives the error bits (0: success) when the kernel ends; may be null
+  bool w_kn = false; // w is [K, N] (N contiguous), e.g. an nn.Linear weight in its own backward pass: C = A * W
 };
 
-// C = A * W^T computed tile by tile on the tensor cores (TMA -> smem ->
+// C = A * W^T (A * W with w_kn) computed tile by tile on the tensor cores (TMA -> smem ->
 // wgmma -> register accumulators); every finished accumulator tile is converted
 // to bf16, staged in shared memory and added straight into its owner rank's
 // output shard over NVLink by the TMA unit (cp.reduce.async.bulk.tensor .add on
@@ -36,14 +37,15 @@ cudaError_t launch_gemm_rs(CudaDevice &dev, const GemmRsArgs &args, cudaStream_t
 
 struct AgGemmArgs {
   uint64_t a_off;        // heap offset of this rank's [M / P, K] bf16 shard of the activations (the same on every rank)
-  const void *w;         // [N, K] bf16 row-major (this rank's output features, nn.Linear layout)
+  const void *w;         // [N, K] bf16 row-major (this rank's output features, nn.Linear layout), or [K, N] with w_kn
   void *gathered;        // [M, K] bf16: receives every rank's shard in rank order
   void *out;             // [M, N] bf16
   uint32_t m, n, k;
   uint32_t *status_dev;  // device word that receives the error bits (0: success) when the kernel ends; may be null
+  bool w_kn = false;     // w is [K, N] (N contiguous), e.g. an nn.Linear weight in its own backward pass: C = A * W
 };
 
-// C = allgather_M(A_shard) * W^T: the first half of a sequence-parallel column-parallel linear layer.  One
+// C = allgather_M(A_shard) * W^T (* W with w_kn): the first half of a sequence-parallel column-parallel linear layer.  One
 // persistent wgmma kernel computes the tiles of this rank's own rows first while spare warps pull the peers'
 // shards over NVLink into `gathered`, 128 rows at a time and in the order the tiles consume them; a tile of peer rows
 // waits only for its own 128 rows.  Throws std::invalid_argument before enqueueing anything unless

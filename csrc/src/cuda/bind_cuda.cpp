@@ -130,32 +130,34 @@ void bind_cuda(py::module_ &m) {
     if (!d) throw std::runtime_error("not a CUDA backend");
     return d->debug_state();
   });
-  // out_shard[M/P, N] (heap buffer, bf16) = reduce_scatter_M( A[M,K] @ W[N,K]^T ), fused on wgmma + NVLink
+  // out_shard[M/P, N] (heap buffer, bf16) = reduce_scatter_M( A[M,K] @ W[N,K]^T ) (or @ W[K,N] with w_kn), fused on wgmma + NVLink
   m.def("gemm_reduce_scatter", [](ACCL &a, uintptr_t a_ptr, uintptr_t w_ptr, BaseBuffer &out, uint32_t M, uint32_t N, uint32_t K,
-                                  uintptr_t stream, int variant, uintptr_t status_dev_ptr) {
+                                  uintptr_t stream, int variant, uintptr_t status_dev_ptr, bool w_kn) {
     auto *d = dynamic_cast<CudaDevice *>(a.device());
     if (!d) throw std::runtime_error("not a CUDA backend");
     GemmRsArgs g{reinterpret_cast<const void *>(a_ptr), reinterpret_cast<const void *>(w_ptr), out.address(), M, N, K, 0};
     g.variant = variant;
     g.out_f32 = out.type() == dataType::float32;
     g.status_dev = reinterpret_cast<uint32_t *>(status_dev_ptr);
+    g.w_kn = w_kn;
     if (!g.out_f32 && out.type() != dataType::bfloat16) throw std::invalid_argument("gemm_reduce_scatter: output shard must be bf16 or fp32");
     cudaError_t e = launch_gemm_rs(*d, g, reinterpret_cast<cudaStream_t>(stream));
     if (e != cudaSuccess) throw std::runtime_error(std::string("gemm_reduce_scatter launch: ") + cudaGetErrorString(e));
   }, py::arg("accl"), py::arg("a_ptr"), py::arg("w_ptr"), py::arg("out"), py::arg("M"), py::arg("N"), py::arg("K"), py::arg("stream"),
-        py::arg("variant") = 0, py::arg("status_dev_ptr") = 0, py::call_guard<py::gil_scoped_release>());
-  // out[M, N] = allgather_M(shard[M/P, K]) @ W[N, K]^T, fused on wgmma + NVLink; gathered[M, K] receives the gathered rows
+        py::arg("variant") = 0, py::arg("status_dev_ptr") = 0, py::arg("w_kn") = false, py::call_guard<py::gil_scoped_release>());
+  // out[M, N] = allgather_M(shard[M/P, K]) @ W[N, K]^T (or @ W[K, N] with w_kn), fused on wgmma + NVLink; gathered[M, K]
+  // receives the gathered rows
   m.def("all_gather_gemm", [](ACCL &a, BaseBuffer &shard, uintptr_t w_ptr, uintptr_t gathered_ptr, uintptr_t out_ptr, uint32_t M,
-                              uint32_t N, uint32_t K, uintptr_t status_dev_ptr, uintptr_t stream) {
+                              uint32_t N, uint32_t K, uintptr_t status_dev_ptr, uintptr_t stream, bool w_kn) {
     auto *d = dynamic_cast<CudaDevice *>(a.device());
     if (!d) throw std::runtime_error("not a CUDA backend");
     if (shard.type() != dataType::bfloat16) throw std::invalid_argument("all_gather_gemm: the shard must be bf16");
     AgGemmArgs g{shard.address(), reinterpret_cast<const void *>(w_ptr), reinterpret_cast<void *>(gathered_ptr),
-                 reinterpret_cast<void *>(out_ptr), M, N, K, reinterpret_cast<uint32_t *>(status_dev_ptr)};
+                 reinterpret_cast<void *>(out_ptr), M, N, K, reinterpret_cast<uint32_t *>(status_dev_ptr), w_kn};
     cudaError_t e = launch_ag_gemm(*d, g, reinterpret_cast<cudaStream_t>(stream));
     if (e != cudaSuccess) throw std::runtime_error(std::string("all_gather_gemm launch: ") + cudaGetErrorString(e));
   }, py::arg("accl"), py::arg("shard"), py::arg("w_ptr"), py::arg("gathered_ptr"), py::arg("out_ptr"), py::arg("M"), py::arg("N"),
-        py::arg("K"), py::arg("status_dev_ptr"), py::arg("stream"), py::call_guard<py::gil_scoped_release>());
+        py::arg("K"), py::arg("status_dev_ptr"), py::arg("stream"), py::arg("w_kn") = false, py::call_guard<py::gil_scoped_release>());
   // out = allreduce_sum(x + y): the kernel computes and then issues the collective itself (device API -> engine)
   m.def("vadd_allreduce", [](ACCL &a, BaseBuffer &x, BaseBuffer &y, BaseBuffer &tmp, BaseBuffer &out, uint32_t count,
                              uintptr_t status_dev_ptr, uintptr_t stream, uint32_t chunk_elems) {

@@ -4,7 +4,9 @@
 // Each rank holds A_r, its [M/P, K] rows of the activations (bf16, in the symmetric heap at the same offset on every
 // rank), and W_r [N_r, K], its output features (bf16, nn.Linear layout).  The op computes
 //   C[M, N_r] = allgather_M(A_r) W_r^T        (bf16 out, fp32 accumulation)
-// and leaves the gathered activations [M, K] in rank order, which backward passes reuse.
+// and leaves the gathered activations [M, K] in rank order, which backward passes reuse.  W_r may also be stored
+// [K, N_r] (N contiguous, AgGemmArgs::w_kn): an nn.Linear weight used in its own backward pass,
+// dX_r = allgather_M(dY_r) W_r.  It is loaded in 64-column boxes and fed to wgmma MN-major (k_plugin_ag_gemm<true>).
 //
 // One persistent, warp-specialised sm_90a kernel per rank, one CTA per 128 x 256 tile on every SM, with the 4-stage
 // TMA -> mbarrier -> wgmma.m64n256k16 pipeline of the single-CTA GEMM -> reduce-scatter kernel (wgmma.cuh):
@@ -97,6 +99,7 @@ __device__ __forceinline__ void copy_slice(const char *src, char *dst, size_t nv
   for (; i < nvec; i += stride) dev::st_stream(dst + i * 16, dev::ld_volatile16(src + i * 16));
 }
 
+template <bool KN>
 __global__ void __launch_bounds__(g::THREADS, 1)
 k_plugin_ag_gemm(const __grid_constant__ CUtensorMap tmap_own, const __grid_constant__ CUtensorMap tmap_gathered,
                  const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_c, AgGemmParams p) {
@@ -220,7 +223,15 @@ k_plugin_ag_gemm(const __grid_constant__ CUtensorMap tmap_own, const __grid_cons
           mbar_wait(&empty[stage], phase ^ 1);
           mbar_expect_tx(&full[stage], STAGE_BYTES);
           tma_load_2d(smem_a + stage * A_STAGE_BYTES, map_a, &full[stage], static_cast<int>(kb * BK), row_a);
-          tma_load_2d(smem_b + stage * B_STAGE_BYTES, &tmap_w, &full[stage], static_cast<int>(kb * BK), static_cast<int>(nb * BN));
+          if constexpr (KN) {
+            // W is [K, N]: boxes of 64 columns x 64 K-rows, one 8 KB column of swizzle atoms each
+#pragma unroll
+            for (int j = 0; j < BN / 64; ++j)
+              tma_load_2d(smem_b + stage * B_STAGE_BYTES + j * (64 * BK * 2), &tmap_w, &full[stage], static_cast<int>(nb * BN + 64 * j),
+                          static_cast<int>(kb * BK));
+          } else {
+            tma_load_2d(smem_b + stage * B_STAGE_BYTES, &tmap_w, &full[stage], static_cast<int>(kb * BK), static_cast<int>(nb * BN));
+          }
         }
         __syncwarp();
         if (++stage == STAGES) {
@@ -247,11 +258,13 @@ k_plugin_ag_gemm(const __grid_constant__ CUtensorMap tmap_own, const __grid_cons
       for (uint32_t kb = 0; kb < k_blocks; ++kb) {
         mbar_wait(&full[stage], phase);
         const uint64_t da = make_smem_desc(smem_u32(smem_a + stage * A_STAGE_BYTES + wg * 64 * 128));
-        const uint64_t db = make_smem_desc(smem_u32(smem_b + stage * B_STAGE_BYTES));
+        const uint32_t b_addr = smem_u32(smem_b + stage * B_STAGE_BYTES);
+        const uint64_t db = KN ? make_smem_desc_mn(b_addr) : make_smem_desc(b_addr);
+        constexpr uint64_t DB_STEP = KN ? 128 : 2; // per K=16 step, >> 4: 16 K-rows of 128 B (MN-major), 32 B (K-major)
         wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < BK / WGMMA_K; ++kk) // +32 bytes (>>4 = 2) per K=16 step inside the swizzle atom
-          wgmma_m64n256k16(d, da + 2 * kk, db + 2 * kk, (kb | kk) ? 1u : 0u);
+        for (int kk = 0; kk < BK / WGMMA_K; ++kk) // A: +32 bytes (>>4 = 2) per K=16 step inside the swizzle atom
+          wgmma_m64n256k16<KN ? 1 : 0>(d, da + 2 * kk, db + DB_STEP * kk, (kb | kk) ? 1u : 0u);
         wgmma_commit();
         wgmma_wait<1>(); // the previous stage's MMAs have retired: it may be refilled
         if (kb > 0 && signaller) mbar_arrive(&empty[prev]);
@@ -294,8 +307,10 @@ std::map<CudaDevice *, unsigned int *> g_ag_flags;
 
 void preload_ag_gemm_kernels() {
   cudaFuncAttributes a;
-  cudaFuncGetAttributes(&a, k_plugin_ag_gemm);
-  cudaFuncSetAttribute(k_plugin_ag_gemm, cudaFuncAttributeMaxDynamicSharedMemorySize, g::SMEM_BYTES);
+  cudaFuncGetAttributes(&a, k_plugin_ag_gemm<false>);
+  cudaFuncGetAttributes(&a, k_plugin_ag_gemm<true>);
+  cudaFuncSetAttribute(k_plugin_ag_gemm<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, g::SMEM_BYTES);
+  cudaFuncSetAttribute(k_plugin_ag_gemm<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, g::SMEM_BYTES);
 }
 
 cudaError_t launch_ag_gemm(CudaDevice &dev, const AgGemmArgs &a, cudaStream_t stream) {
@@ -323,7 +338,7 @@ cudaError_t launch_ag_gemm(CudaDevice &dev, const AgGemmArgs &a, cudaStream_t st
   }
   const CUtensorMap t_own = make_map(w.window + static_cast<uint64_t>(w.rank) * w.heap_bytes + a.a_off, a.m / P, a.k, BM, BK);
   const CUtensorMap t_gathered = make_map(a.gathered, a.m, a.k, BM, BK);
-  const CUtensorMap t_w = make_map(a.w, a.n, a.k, BN, BK);
+  const CUtensorMap t_w = a.w_kn ? make_map(a.w, a.k, a.n, BK, 64) : make_map(a.w, a.n, a.k, BN, BK);
   const CUtensorMap t_c = make_map(a.out, a.m, a.n, EPI_ROWS, 64);
   AgGemmParams p;
   p.w = w;
@@ -339,14 +354,15 @@ cudaError_t launch_ag_gemm(CudaDevice &dev, const AgGemmArgs &a, cudaStream_t st
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev.device());
   ACCL_CUDART(cudaMemsetAsync(flags, 0, AG_FLAG_WORDS * sizeof(unsigned int), stream));
   const uint32_t tiles = (a.m / BM) * (a.n / BN);
-  cudaFuncSetAttribute(k_plugin_ag_gemm, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+  const auto kernel = a.w_kn ? k_plugin_ag_gemm<true> : k_plugin_ag_gemm<false>;
+  cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
   cudaLaunchConfig_t lc = {};
   // every CTA copies a slice of every chunk and waits for the others' slices: the whole grid must be resident, one CTA per SM
   lc.gridDim = dim3(std::min<uint32_t>(static_cast<uint32_t>(sms), tiles));
   lc.blockDim = dim3(THREADS);
   lc.dynamicSmemBytes = SMEM_BYTES;
   lc.stream = stream;
-  return cudaLaunchKernelEx(&lc, k_plugin_ag_gemm, t_own, t_gathered, t_w, t_c, p);
+  return cudaLaunchKernelEx(&lc, kernel, t_own, t_gathered, t_w, t_c, p);
 }
 
 } // namespace cuda

@@ -3,6 +3,8 @@
 // Each rank holds a K-slice of a row-parallel linear layer: A_r [M, K_r] and
 // W_r [N, K_r] (bf16, K contiguous).  The full product is C = sum_r A_r W_r^T,
 // reduce-scattered along M: rank o ends up with rows [o*M/P, (o+1)*M/P).
+// W_r may also be stored [K_r, N] (N contiguous, GemmRsArgs::w_kn): an nn.Linear weight used in its own backward
+// pass, dX = RS_M(dY W).  It is loaded in 64-column boxes and fed to wgmma MN-major (KN kernels); nothing else changes.
 //
 // One persistent, warp-specialised sm_90a kernel per rank, in two flavours selected at run time
 // (GemmRsArgs::variant, default: the CTA pair when the shape allows it):
@@ -116,7 +118,7 @@ __device__ __forceinline__ void emit_chunks(const float (&d)[128], uint8_t *my_e
   }
 }
 
-template <bool PAIR, bool F32>
+template <bool PAIR, bool F32, bool KN>
 __global__ void __launch_bounds__(g::THREADS, 1)
 k_plugin_gemm_rs(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                  const __grid_constant__ OutMaps out_maps, GemmRsParams p) {
@@ -226,11 +228,23 @@ k_plugin_gemm_rs(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
           mbar_expect_tx(&full[stage], STAGE_BYTES);
           tma_load_2d(smem_a + stage * A_STAGE_BYTES, &tmap_a, &full[stage], static_cast<int>(kb * BK),
                       static_cast<int>(mb * C::TILE_M + cr * BM));
-          if (PAIR)
+          if constexpr (KN) {
+            // W is [K, N]: this CTA's columns in boxes of 64 columns x 64 K-rows, one 8 KB column of swizzle atoms each
+#pragma unroll
+            for (int j = 0; j < C::BN_LOAD / 64; ++j) {
+              uint8_t *dst = smem_b + stage * B_STAGE_BYTES + cr * (C::BN_LOAD * BK * 2) + j * (64 * BK * 2);
+              const int n0 = static_cast<int>(nb * BN + cr * C::BN_LOAD + 64 * j), k0 = static_cast<int>(kb * BK);
+              if (PAIR)
+                tma_load_2d_multicast(dst, &tmap_b, &full[stage], n0, k0, 0x3);
+              else
+                tma_load_2d(dst, &tmap_b, &full[stage], n0, k0);
+            }
+          } else if (PAIR) {
             tma_load_2d_multicast(smem_b + stage * B_STAGE_BYTES + cr * (C::BN_LOAD * BK * 2), &tmap_b, &full[stage],
                                   static_cast<int>(kb * BK), static_cast<int>(nb * BN + cr * C::BN_LOAD), 0x3);
-          else
+          } else {
             tma_load_2d(smem_b + stage * B_STAGE_BYTES, &tmap_b, &full[stage], static_cast<int>(kb * BK), static_cast<int>(nb * BN));
+          }
         }
         __syncwarp();
         if (++stage == STAGES) {
@@ -264,11 +278,13 @@ k_plugin_gemm_rs(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       for (uint32_t kb = 0; kb < k_blocks; ++kb) {
         mbar_wait(&full[stage], phase);
         const uint64_t da = make_smem_desc(smem_u32(smem_a + stage * A_STAGE_BYTES + wg * 64 * 128));
-        const uint64_t db = make_smem_desc(smem_u32(smem_b + stage * B_STAGE_BYTES));
+        const uint32_t b_addr = smem_u32(smem_b + stage * B_STAGE_BYTES);
+        const uint64_t db = KN ? make_smem_desc_mn(b_addr) : make_smem_desc(b_addr);
+        constexpr uint64_t DB_STEP = KN ? 128 : 2; // per K=16 step, >> 4: 16 K-rows of 128 B (MN-major), 32 B (K-major)
         wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < BK / WGMMA_K; ++kk) // +32 bytes (>>4 = 2) per K=16 step inside the swizzle atom
-          wgmma_m64n256k16(d, da + 2 * kk, db + 2 * kk, (kb | kk) ? 1u : 0u);
+        for (int kk = 0; kk < BK / WGMMA_K; ++kk) // A: +32 bytes (>>4 = 2) per K=16 step inside the swizzle atom
+          wgmma_m64n256k16<KN ? 1 : 0>(d, da + 2 * kk, db + DB_STEP * kk, (kb | kk) ? 1u : 0u);
         wgmma_commit();
         wgmma_wait<1>(); // the previous stage's MMAs have retired: it may be refilled
         if (kb > 0) release(prev);
@@ -329,28 +345,32 @@ struct PluginState {
 std::mutex g_state_m;
 std::map<CudaDevice *, PluginState> g_state;
 
-template <bool PAIR, bool F32> void set_smem_attr() {
-  cudaFuncSetAttribute(k_plugin_gemm_rs<PAIR, F32>, cudaFuncAttributeMaxDynamicSharedMemorySize, g::SMEM_BYTES);
+template <bool PAIR, bool F32, bool KN> void set_smem_attr() {
+  cudaFuncSetAttribute(k_plugin_gemm_rs<PAIR, F32, KN>, cudaFuncAttributeMaxDynamicSharedMemorySize, g::SMEM_BYTES);
+}
+template <bool KN> void preload_layout() {
+  cudaFuncAttributes a;
+  cudaFuncGetAttributes(&a, k_plugin_gemm_rs<false, false, KN>);
+  cudaFuncGetAttributes(&a, k_plugin_gemm_rs<false, true, KN>);
+  cudaFuncGetAttributes(&a, k_plugin_gemm_rs<true, false, KN>);
+  cudaFuncGetAttributes(&a, k_plugin_gemm_rs<true, true, KN>);
+  set_smem_attr<false, false, KN>();
+  set_smem_attr<false, true, KN>();
+  set_smem_attr<true, false, KN>();
+  set_smem_attr<true, true, KN>();
 }
 } // namespace
 
 void preload_gemm_rs_kernels() {
-  cudaFuncAttributes a;
-  cudaFuncGetAttributes(&a, k_plugin_gemm_rs<false, false>);
-  cudaFuncGetAttributes(&a, k_plugin_gemm_rs<false, true>);
-  cudaFuncGetAttributes(&a, k_plugin_gemm_rs<true, false>);
-  cudaFuncGetAttributes(&a, k_plugin_gemm_rs<true, true>);
-  set_smem_attr<false, false>();
-  set_smem_attr<false, true>();
-  set_smem_attr<true, false>();
-  set_smem_attr<true, true>();
+  preload_layout<false>();
+  preload_layout<true>();
 }
 
-template <bool PAIR, bool F32>
+template <bool PAIR, bool F32, bool KN>
 static cudaError_t launch_variant(const CUtensorMap &ta, const CUtensorMap &tb, const OutMaps &om, const GemmRsParams &p, uint32_t tiles,
                                   int sms, cudaStream_t stream) {
   using namespace g;
-  set_smem_attr<PAIR, F32>();
+  set_smem_attr<PAIR, F32, KN>();
   cudaLaunchConfig_t lc = {};
   lc.blockDim = dim3(THREADS);
   lc.dynamicSmemBytes = SMEM_BYTES;
@@ -367,13 +387,13 @@ static cudaError_t launch_variant(const CUtensorMap &ta, const CUtensorMap &tb, 
     lc.gridDim = dim3(2 * pairs);
     // the kernel spins on grid-wide flags: every cluster must be resident at once
     int max_clusters = 0;
-    if (cudaOccupancyMaxActiveClusters(&max_clusters, k_plugin_gemm_rs<PAIR, F32>, &lc) == cudaSuccess && max_clusters > 0)
+    if (cudaOccupancyMaxActiveClusters(&max_clusters, k_plugin_gemm_rs<PAIR, F32, KN>, &lc) == cudaSuccess && max_clusters > 0)
       pairs = std::min<uint32_t>(pairs, static_cast<uint32_t>(max_clusters));
     lc.gridDim = dim3(2 * pairs);
   } else {
     lc.gridDim = dim3(std::min<uint32_t>(static_cast<uint32_t>(sms), tiles));
   }
-  return cudaLaunchKernelEx(&lc, k_plugin_gemm_rs<PAIR, F32>, ta, tb, om, p);
+  return cudaLaunchKernelEx(&lc, k_plugin_gemm_rs<PAIR, F32, KN>, ta, tb, om, p);
 }
 
 cudaError_t launch_gemm_rs(CudaDevice &dev, const GemmRsArgs &a, cudaStream_t stream) {
@@ -403,7 +423,8 @@ cudaError_t launch_gemm_rs(CudaDevice &dev, const GemmRsArgs &a, cudaStream_t st
   const bool pair = variant == 2 || (variant == 0 && pair_ok);
   const bool f32 = a.out_f32;
   const CUtensorMap ta = make_map(a.a, a.m, a.k, BM, BK);
-  const CUtensorMap tb = make_map(a.w, a.n, a.k, pair ? BN / 2 : BN, BK); // each CTA of a pair loads half of the N tile
+  // each CTA of a pair loads half of the N tile; a [K, N] weight goes in boxes of 64 columns x 64 K-rows
+  const CUtensorMap tb = a.w_kn ? make_map(a.w, a.k, a.n, BK, 64) : make_map(a.w, a.n, a.k, pair ? BN / 2 : BN, BK);
   OutMaps om;
   std::memset(&om, 0, sizeof(om));
   for (uint32_t o = 0; o < P; ++o) // symmetric allocation: the shard sits at out_off in every heap (verified in-kernel:
@@ -424,8 +445,12 @@ cudaError_t launch_gemm_rs(CudaDevice &dev, const GemmRsArgs &a, cudaStream_t st
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev.device());
   ACCL_CUDART(cudaMemsetAsync(st->flags, 0, 64 * sizeof(unsigned int), stream));
   const uint32_t tiles = (a.m / (pair ? 2 * BM : BM)) * (a.n / BN);
-  if (pair) return f32 ? launch_variant<true, true>(ta, tb, om, p, tiles, sms, stream) : launch_variant<true, false>(ta, tb, om, p, tiles, sms, stream);
-  return f32 ? launch_variant<false, true>(ta, tb, om, p, tiles, sms, stream) : launch_variant<false, false>(ta, tb, om, p, tiles, sms, stream);
+  if (a.w_kn) {
+    if (pair) return f32 ? launch_variant<true, true, true>(ta, tb, om, p, tiles, sms, stream) : launch_variant<true, false, true>(ta, tb, om, p, tiles, sms, stream);
+    return f32 ? launch_variant<false, true, true>(ta, tb, om, p, tiles, sms, stream) : launch_variant<false, false, true>(ta, tb, om, p, tiles, sms, stream);
+  }
+  if (pair) return f32 ? launch_variant<true, true, false>(ta, tb, om, p, tiles, sms, stream) : launch_variant<true, false, false>(ta, tb, om, p, tiles, sms, stream);
+  return f32 ? launch_variant<false, true, false>(ta, tb, om, p, tiles, sms, stream) : launch_variant<false, false, false>(ta, tb, om, p, tiles, sms, stream);
 }
 
 } // namespace cuda

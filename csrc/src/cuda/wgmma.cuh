@@ -71,13 +71,27 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
   return d;
 }
 
+// MN-major, 128B-swizzled descriptor for a B operand stored [K, N] (N contiguous) and loaded as boxes of 64 columns x
+// 64 K-rows: a swizzle atom is 8 K-rows of 128 bytes (64 columns); atoms along N sit one box (8 KB, leading byte
+// offset) apart, 8-row groups along K 1 KB (stride byte offset) apart.  One K=16 step is 16 rows = 2048 bytes.
+__device__ __forceinline__ uint64_t make_smem_desc_mn(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);      // start address >> 4
+  d |= static_cast<uint64_t>(8192 >> 4) << 16;                  // leading byte offset: next 64 columns
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;                  // stride byte offset: next 8 K-rows
+  d |= static_cast<uint64_t>(1) << 62;                          // SWIZZLE_128B
+  return d;
+}
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// D[64 x 256] (+)= A[64 x 16] B[256 x 16]^T, bf16 operands K-major in smem, fp32 D in registers (warpgroup-wide).
+// D[64 x 256] (+)= A[64 x 16] B[256 x 16]^T, bf16 operands in smem, fp32 D in registers (warpgroup-wide).  A is
+// K-major; B is K-major (TNSP_B = 0, desc_b from make_smem_desc) or MN-major (TNSP_B = 1, make_smem_desc_mn).
 // Thread t of the warpgroup holds rows 16*(t/32) + (t%32)/4 (+8) and columns 8*j + 2*(t%4) (+1), j = 0..31:
 // d[4j], d[4j+1] on the first row, d[4j+2], d[4j+3] on the second.
+template <int TNSP_B = 0>
 __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
       "{\n"
@@ -92,7 +106,7 @@ __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t desc_
       "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
       "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
       "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
-      "%128, %129, p, 1, 1, 0, 0;\n"
+      "%128, %129, p, 1, 1, 0, %131;\n"
       "}\n"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
         "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
@@ -110,7 +124,7 @@ __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t desc_
         "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
         "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
         "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
-      : "l"(desc_a), "l"(desc_b), "r"(accumulate)
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(TNSP_B)
       : "memory");
 }
 

@@ -35,25 +35,28 @@ EXCERPTS = [
     ("persistent engine: command fetch / parked-call loop of the control CTA", "k_engine", r"NANOSLEEP", 20, 20,
      "the control CTA polls the command ring with `ld.acquire.sys`, steps every call in flight and backs off with NANOSLEEP "
      "only after 100 us without work."),
-    ("wgmma GEMM: MMA issue loop", "k_plugin_gemm_rs_true_false", r"HGMMA\.64x256x16", 6, 30,
+    ("wgmma GEMM: MMA issue loop", "k_plugin_gemm_rs_true_false_false", r"HGMMA\.64x256x16", 6, 30,
      "`wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16` from shared-memory descriptors, issued by each consumer "
      "warpgroup into its register accumulators."),
-    ("wgmma GEMM, CTA pair: TMA loads", "k_plugin_gemm_rs_true_false", r"UTMALDG\.2D\.MULTICAST", 4, 10,
+    ("wgmma GEMM, CTA pair: TMA loads", "k_plugin_gemm_rs_true_false_false", r"UTMALDG\.2D\.MULTICAST", 4, 10,
      "`cp.async.bulk.tensor.2d ... multicast::cluster`: each CTA of the pair loads half of the W tile into both CTAs."),
-    ("wgmma GEMM epilogue: registers -> swizzled smem -> TMA reduce-add into the owner rank's shard", "k_plugin_gemm_rs_true_false",
+    ("wgmma GEMM epilogue: registers -> swizzled smem -> TMA reduce-add into the owner rank's shard", "k_plugin_gemm_rs_true_false_false",
      r"UTMAREDG\.2D\.ADD", 30, 6,
      "`UTMAREDG.2D.ADD` = `cp.reduce.async.bulk.tensor.2d ... .add`: the tile is added into "
      "peer memory over NVLink by the TMA unit (device API `reduce_scatter_emit_tile`)."),
-    ("all-gather -> GEMM: MMA issue loop", "k_plugin_ag_gemm", r"HGMMA\.64x256x16", 6, 30,
+    ("all-gather -> GEMM: MMA issue loop", "k_plugin_ag_gemm_false", r"HGMMA\.64x256x16", 6, 30,
      "the same m64n256k16 wgmma mainloop as the single-CTA GEMM -> reduce-scatter, on A tiles of own rows from the local "
      "shard and of peer rows from `gathered`."),
-    ("all-gather -> GEMM: pull loop over the peer-mapped heap", "k_plugin_ag_gemm", r"LDG\.E\.128\.STRONG\.SYS", 4, 24,
+    ("all-gather -> GEMM: pull loop over the peer-mapped heap", "k_plugin_ag_gemm_false", r"LDG\.E\.128\.STRONG\.SYS", 4, 24,
      "`ld.volatile.global.v4.u32` from the peer's shard through its heap window, four loads in flight per thread before "
      "their `STG.E.NA.128` stores into the local `gathered` rows."),
-    ("all-gather -> GEMM epilogue: registers -> swizzled smem -> TMA tensor store into C", "k_plugin_ag_gemm",
+    ("all-gather -> GEMM epilogue: registers -> swizzled smem -> TMA tensor store into C", "k_plugin_ag_gemm_false",
      r"UTMASTG\.2D", 30, 6,
      "`UTMASTG.2D` = `cp.async.bulk.tensor.2d.global.shared::cta.bulk_group`: the bf16 tile leaves shared memory for the "
      "local C through the TMA unit."),
+    ("wgmma GEMM with a [K, N] weight: MMA issue loop", "k_plugin_gemm_rs_true_false_true", r"HGMMA\.64x256x16", 6, 30,
+     "the same instruction with `.tnspB`: B is read MN-major from 64-column boxes of the [K, N] weight (an nn.Linear "
+     "weight in its own backward pass), the descriptor advancing 2048 bytes per K=16 step."),
 ]
 
 
