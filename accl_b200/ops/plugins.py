@@ -4,6 +4,9 @@
   K-slice on the tensor cores (wgmma) and each finished tile is added straight
   into the owner rank's output shard over NVLink (no intermediate C, no
   separate reduce_scatter kernel).
+* gemm_all_reduce: the same GEMM whose epilogue is an all-reduce — each tile is
+  added into its owner rank over NVLink, and the owner copies the finished tile
+  into every peer, so every rank ends with the same full C.
 * all_gather_gemm: the column-parallel counterpart — the GEMM starts on this
   rank's own rows while the kernel pulls the peers' shards over NVLink, and
   each peer tile waits only for its own 128 rows.
@@ -74,6 +77,75 @@ def gemm_reduce_scatter(accl: Accl, a: torch.Tensor, w: torch.Tensor, out: Buffe
     status_ptr = _status_ptr("gemm_reduce_scatter", status, device)
     _C.gemm_reduce_scatter(accl.impl, a.data_ptr(), w.data_ptr(), out.impl, M, N, K, _stream_handle(accl), variant,
                            status_ptr, kn)
+    return out
+
+
+GEMM_AR_MAX_TILES = 16384  # plugins.hpp: most 128 x 256 tiles of one gemm_all_reduce call
+
+
+def _gemm_ar_counters(accl: Accl) -> Buffer:
+    """The heap block of per-tile arrival counters gemm_all_reduce signals in, allocated at this Accl's first call (in
+    the same order on every rank, so at the same offset) and kept; the kernel verifies the offsets match."""
+    cnt = getattr(accl, "_gemm_ar_counters", None)
+    if cnt is None:
+        cnt = accl._gemm_ar_counters = accl.create_buffer(GEMM_AR_MAX_TILES, torch.int32)
+    return cnt
+
+
+def gemm_all_reduce(accl: Accl, a: torch.Tensor, w: torch.Tensor, out: Buffer = None, variant: int = 0, out_dtype=None,
+                    status: torch.Tensor = None, w_layout: str = "nk") -> Buffer:
+    """out[M, N] (in the symmetric heap) = all_reduce over ranks of a[M, K_r] @ w[N, K_r]^T, the same bits on every rank.
+
+    `a` and `w` are this rank's K-slices (bf16, contiguous, on this rank's GPU).  w_layout "nk" (default): `w` is
+    [N, K_r] (nn.Linear layout); "kn": `w` is [K_r, N] and the product is a @ w, e.g. an nn.Linear weight in its own
+    backward pass, dX = all_reduce(dY @ W), without a transposed copy.
+    Needs M % 128 == 0, N % 256 == 0, K_r % 64 == 0 and (M / 128) (N / 256) <= 16384 tiles.  Stream ordered.
+    One kernel: every rank adds its partial of each 128 x 256 (or 256 x 256) tile into the tile's owner rank over
+    NVLink, and the owner copies the finished tile into every peer's `out`, so all replicas are bit-identical.
+    `out` is bf16 (partials added in bf16 by the TMA unit) or, with an fp32 `out` buffer / out_dtype, fp32 (the P
+    partial products are accumulated without intermediate rounding); out_dtype defaults to `out`'s dtype, or bf16.
+    `out` must sit at the same heap offset on every rank: allocate it in the same order everywhere.
+    variant: 0 automatic, 1 one CTA per 128 x 256 tile, 2 CTA pair per 256 x 256 tile (needs M % 256 == 0).
+    `status`, optional 1-element int32 CUDA tensor, receives the error bits when the kernel ends (0: success); with
+    non-zero bits `out` is not a valid result.  An `out` at a different heap offset on some peer sets
+    DMA_MISMATCH_ERROR (bit 0) on both ranks, and neither writes into the other's heap.
+    Raises ValueError for a wrong dtype, shape, layout or device, too many tiles, or an `out` that is not a large
+    enough heap buffer.
+    """
+    op = "gemm_all_reduce"
+    device = torch.device("cuda", accl.cuda_device)
+    _check_operand(op, "a", a, device)
+    _check_operand(op, "w", w, device)
+    kn = _is_kn(op, w_layout)
+    M, K = a.shape
+    N, w_k = (w.shape[1], w.shape[0]) if kn else (w.shape[0], w.shape[1])
+    if w_k != K:
+        raise ValueError(f"{op}: w has K = {w_k}, a has K = {K}")
+    if M % 128 or N % 256 or K % 64 or not (M and N and K):
+        raise ValueError(f"{op}: need M % 128 == 0, N % 256 == 0, K % 64 == 0, none of them zero; got M = {M}, N = {N}, K = {K}")
+    if (M // 128) * (N // 256) > GEMM_AR_MAX_TILES:
+        raise ValueError(f"{op}: M = {M}, N = {N} is {(M // 128) * (N // 256)} tiles of 128 x 256, more than {GEMM_AR_MAX_TILES}")
+    if variant not in (0, 1, 2):
+        raise ValueError(f"{op}: variant must be 0, 1 or 2, got {variant}")
+    if variant == 2 and M % 256:
+        raise ValueError(f"{op}: the CTA-pair variant needs M % 256 == 0, got M = {M}")
+    if out_dtype not in (None, torch.bfloat16, torch.float32):
+        raise ValueError(f"{op}: out_dtype must be torch.bfloat16 or torch.float32, got {out_dtype}")
+    if out is not None and (not isinstance(out, Buffer) or not accl.heap_contains(_device_view(out))):
+        raise ValueError(f"{op}: out must be a buffer in the symmetric heap (accl.create_buffer)")
+    if out is not None:
+        dt = to_torch(out.dtype)
+        if dt not in (torch.bfloat16, torch.float32) or (out_dtype is not None and dt != out_dtype):
+            raise ValueError(f"{op}: out is {dt}; it must be bf16 or fp32"
+                             + (f" and match out_dtype = {out_dtype}" if out_dtype is not None else ""))
+        if out.length < M * N:
+            raise ValueError(f"{op}: out holds {out.length} elements, the result needs {M * N}")
+    status_ptr = _status_ptr(op, status, device)
+    counters = _gemm_ar_counters(accl)
+    if out is None:
+        out = accl.create_buffer(M * N, out_dtype or torch.bfloat16)
+    _C.gemm_all_reduce(accl.impl, a.data_ptr(), w.data_ptr(), out.impl, counters.impl, M, N, K, _stream_handle(accl),
+                       variant, status_ptr, kn)
     return out
 
 

@@ -16,6 +16,9 @@ them on a H100 node:
 * `SeqParallelColumnLinear`  its counterpart: TP column-parallel linear on a sequence-parallel input whose all-gather
                          feeds the GEMM inside one kernel (wgmma plugin); its input gradient runs on the
                          reduce-scatter plugin
+* `ReplicatedRowParallelLinear` / `ReplicatedColumnParallelLinear`  the same pair with activations replicated on every
+                         rank (plain Megatron TP): the row layer's forward and the column layer's input gradient end
+                         in an all-reduce that runs inside the GEMM (accl_b200.ops.gemm_all_reduce)
 * `ring_exchange`        neighbour send/recv step for context-parallel / ring-attention schedules
 * `process_group`        `torch.distributed` backend "accl" (import accl_b200.parallel.process_group): the standard
                          ProcessGroup interface incl. DistributedDataParallel on top of this library
@@ -28,6 +31,7 @@ import torch
 
 from .. import _C
 from ..core import Accl, Buffer, SUM, cuda_rank, socket_rank
+from ..ops.plugins import GEMM_AR_MAX_TILES
 from ..utils.dtypes import to_accl
 
 
@@ -327,6 +331,24 @@ def column_backward_fused(cuda, comm_id, dtype, m, world, in_features, out_featu
             out_features_per_rank % 64 == 0)
 
 
+def _ar_fits(m, n):
+    return m % 128 == 0 and n % 256 == 0 and (m // 128) * (n // 256) <= GEMM_AR_MAX_TILES
+
+
+def row_ar_forward_fused(cuda, comm_id, dtype, m, out_features, in_features_per_rank):
+    """Whether ReplicatedRowParallelLinear's forward runs on ops.gemm_all_reduce: all_reduce([m, K_r] @ [N, K_r]^T).
+    Decode-sized m < 128 and every m % 128 != 0 take matmul + all_reduce."""
+    return (cuda and comm_id == 0 and dtype == torch.bfloat16 and _ar_fits(m, out_features) and
+            in_features_per_rank % 64 == 0)
+
+
+def column_ar_backward_fused(cuda, comm_id, dtype, m, in_features, out_features_per_rank):
+    """Whether ReplicatedColumnParallelLinear's input gradient runs on ops.gemm_all_reduce: dX = all_reduce(dY [m, N_r]
+    @ W_r), the weight [N_r, K] read as [K, N] ("kn"): output columns K % 256, contraction N_r % 64."""
+    return (cuda and comm_id == 0 and dtype == torch.bfloat16 and _ar_fits(m, in_features) and
+            out_features_per_rank % 64 == 0)
+
+
 def _heap_buffer(layer, attr, n):
     """The layer's heap buffer `attr` of n bf16 elements, (re)allocated here: in forward, in the rank's own thread and
     in layer order, so it sits at the same heap offset on every rank."""
@@ -513,6 +535,126 @@ class SeqParallelColumnLinear(torch.nn.Module):
         full = torch.empty(m * P, k, dtype=x.dtype, device=x.device)
         self.group.all_gather_into_tensor(full, x.contiguous())
         return full @ weight.t(), full
+
+
+class _ReplicatedRowFn(torch.autograd.Function):
+    """y = all_reduce(x_r W_r^T); dX_r = dY W_r, dW_r = dY^T x_r (dY is replicated: no communication)."""
+
+    @staticmethod
+    def forward(ctx, x, weight, layer):
+        ctx.save_for_backward(x, weight)
+        return layer._forward(x, weight, training=True)
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, weight = ctx.saved_tensors
+        dx = dy @ weight if ctx.needs_input_grad[0] else None
+        dw = dy.t() @ x if ctx.needs_input_grad[1] else None
+        return dx, dw, None
+
+
+class _ReplicatedColumnFn(torch.autograd.Function):
+    """y_r = x W_r^T; dX = all_reduce(dY_r W_r), dW_r = dY_r^T x."""
+
+    @staticmethod
+    def forward(ctx, x, weight, layer):
+        group = layer.group
+        m, k = x.shape
+        cuda = bool(group.accl.is_cuda)
+        ctx.layer, ctx.m = layer, m
+        ctx.bwd_fused = column_ar_backward_fused(cuda, group.comm_id, _dtype_of(x, weight), m, k, weight.shape[0])
+        ctx.dx_buf = _heap_buffer(layer, "_dx", m * k) if ctx.bwd_fused and ctx.needs_input_grad[0] else None
+        ctx.save_for_backward(x, weight)
+        return x @ weight.t()
+
+    @staticmethod
+    def backward(ctx, dy):
+        from ..ops import gemm_all_reduce
+        x, weight = ctx.saved_tensors
+        group = ctx.layer.group
+        dy = dy.contiguous()
+        dx = None
+        if ctx.needs_input_grad[0]:
+            if ctx.dx_buf is not None:
+                st = group.plugin_status()
+                gemm_all_reduce(group.accl, dy, weight.detach(), ctx.dx_buf, status=st, w_layout="kn")
+                group.note_plugin_status(st)
+                # the heap buffer is rewritten by the next backward through this layer
+                dx = ctx.dx_buf.dev.view(ctx.m, weight.shape[1]).clone()
+            else:
+                dx = (dy @ weight).contiguous()
+                group.all_reduce(dx)
+        dw = dy.t() @ x if ctx.needs_input_grad[1] else None
+        return dx, dw, None
+
+
+class ReplicatedRowParallelLinear(torch.nn.Module):
+    """y = all_reduce_over_ranks(x_r @ W_r^T): Megatron row-parallel linear whose output [m, out_features] is replicated
+    on every rank (the non-sequence-parallel counterpart of `RowParallelLinear`).  On the CUDA backend (bf16, m % 128 ==
+    0, out_features % 256 == 0, in_features_per_rank % 64 == 0, `row_ar_forward_fused`) the all-reduce runs inside the
+    GEMM (accl_b200.ops.gemm_all_reduce) into a heap buffer the layer keeps, and every rank gets the same bits;
+    elsewhere (emulator, fp32, decode-sized m < 128) it falls back to matmul + all_reduce.
+    Trainable: dX_r = dY @ W_r and dW_r = dY^T @ x_r are local matmuls.  Every rank must build its layers and run them
+    in the same order (the heap buffer sits at the same offset on every rank), and fused-call errors surface at
+    `group.check(block=True)` / `group.barrier()`."""
+
+    def __init__(self, group: TensorGroup, in_features_per_rank, out_features, dtype=torch.bfloat16, device=None):
+        super().__init__()
+        self.group = group
+        dev = device if device is not None else (torch.device("cuda", group.accl.cuda_device) if group.accl.is_cuda else "cpu")
+        self.weight = torch.nn.Parameter(torch.empty(out_features, in_features_per_rank, dtype=dtype, device=dev))
+        torch.nn.init.normal_(self.weight, std=0.02)
+        self._out = None
+
+    def forward(self, x):
+        if _wants_grad(x, self.weight):
+            return _ReplicatedRowFn.apply(x, self.weight, self)
+        with torch.no_grad():
+            return self._forward(x, self.weight)
+
+    def _forward(self, x, weight, training=False):
+        """training: the fused call reports into the group's status word, and the result is copied out of the layer's
+        heap buffer, which the next call rewrites (micro-batches, recomputation)."""
+        from ..ops import gemm_all_reduce
+        m, k = x.shape
+        n = weight.shape[0]
+        g = self.group
+        if row_ar_forward_fused(bool(g.accl.is_cuda), g.comm_id, _dtype_of(x, weight), m, n, k):
+            out = _heap_buffer(self, "_out", m * n)
+            if training:
+                st = g.plugin_status()
+                gemm_all_reduce(g.accl, x.contiguous(), weight.detach(), out, status=st)
+                g.note_plugin_status(st)
+                return out.dev.view(m, n).clone()
+            gemm_all_reduce(g.accl, x.contiguous(), weight.data, out)
+            return out.dev.view(m, n)
+        y = (x @ weight.t()).contiguous()
+        g.all_reduce(y)
+        return y
+
+
+class ReplicatedColumnParallelLinear(torch.nn.Module):
+    """y_r = x @ W_r^T: Megatron column-parallel linear on an input [m, in_features] replicated on every rank; returns
+    this rank's [m, out_features_per_rank] features with no communication in forward (the non-sequence-parallel
+    counterpart of `SeqParallelColumnLinear`).  Trainable: the input gradient dX = all_reduce(dY_r @ W_r) runs on
+    accl_b200.ops.gemm_all_reduce reading W_r as [K, N] (no transposed copy) when the shape allows it
+    (`column_ar_backward_fused`), else on matmul + all_reduce; dW_r = dY_r^T @ x is a local matmul.  Every rank must
+    build its layers and run them in the same order, and fused-call errors surface at `group.check(block=True)` /
+    `group.barrier()`."""
+
+    def __init__(self, group: TensorGroup, in_features, out_features_per_rank, dtype=torch.bfloat16, device=None):
+        super().__init__()
+        self.group = group
+        dev = device if device is not None else (torch.device("cuda", group.accl.cuda_device) if group.accl.is_cuda else "cpu")
+        self.weight = torch.nn.Parameter(torch.empty(out_features_per_rank, in_features, dtype=dtype, device=dev))
+        torch.nn.init.normal_(self.weight, std=0.02)
+        self._dx = None  # heap buffer of the fused backward's all-reduced input gradient
+
+    def forward(self, x):
+        if _wants_grad(x, self.weight):
+            return _ReplicatedColumnFn.apply(x, self.weight, self)
+        with torch.no_grad():
+            return x @ self.weight.t()
 
 
 def ring_exchange(group: TensorGroup, send_t: torch.Tensor, recv_t: torch.Tensor, tag=0):

@@ -35,6 +35,31 @@ struct GemmRsArgs {
 // result.  Returns after enqueueing.
 cudaError_t launch_gemm_rs(CudaDevice &dev, const GemmRsArgs &args, cudaStream_t stream);
 
+// most 128 x 256 tiles of one GEMM -> all-reduce call: the size of its counter block, in uint32 words
+constexpr uint32_t GEMM_AR_MAX_TILES = 16384;
+
+struct GemmArArgs {
+  const void *a;     // [M, K] bf16 row-major (this rank's K-slice of the activations)
+  const void *w;     // [N, K] bf16 row-major (this rank's K-slice of the weight, nn.Linear layout), or [K, N] with w_kn
+  uint64_t out_off;  // heap offset of the full [M, N] result (bf16, or fp32 with out_f32), the same on every rank
+  uint64_t cnt_off;  // heap offset of GEMM_AR_MAX_TILES uint32 arrival counters, the same on every rank
+  uint32_t m, n, k;
+  int variant = 0;   // 0: automatic, 1: one CTA per 128 x 256 tile, 2: CTA pair per 256 x 256 tile (M % 256 == 0)
+  bool out_f32 = false; // C is fp32: the P partial products are added without intermediate rounding
+  uint32_t *status_dev = nullptr; // device word that receives the error bits (0: success) when the kernel ends; may be null
+  bool w_kn = false; // w is [K, N] (N contiguous): C = sum_r A_r W_r
+};
+
+// C = sum over ranks of A_r * W_r^T (A_r * W_r with w_kn), the same bits in every rank's heap at out_off: the GEMM ->
+// reduce-scatter kernel with a two-shot all-reduce epilogue.  Every tile has one owner rank; each rank adds its
+// partial tile into the owner's C (TMA reduce-add over NVLink) and signals a per-tile counter in the owner's heap, and
+// the owner copies each complete tile into every peer's C.  C and the counter block must sit at the same offsets on
+// every rank: a peer where either differs gets no adds and no copies, and the call reports DMA_MISMATCH_ERROR.  With
+// non-zero status bits C is not a valid result.  Throws std::invalid_argument before enqueueing anything unless
+// M % 128 == 0 (256 for the CTA pair), N % 256 == 0, K % 64 == 0, (M / 128) (N / 256) <= GEMM_AR_MAX_TILES and both
+// regions are 16-byte aligned inside the heap.  Returns after enqueueing.
+cudaError_t launch_gemm_ar(CudaDevice &dev, const GemmArArgs &args, cudaStream_t stream);
+
 struct AgGemmArgs {
   uint64_t a_off;        // heap offset of this rank's [M / P, K] bf16 shard of the activations (the same on every rank)
   const void *w;         // [N, K] bf16 row-major (this rank's output features, nn.Linear layout), or [K, N] with w_kn

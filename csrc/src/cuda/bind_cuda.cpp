@@ -145,6 +145,24 @@ void bind_cuda(py::module_ &m) {
     if (e != cudaSuccess) throw std::runtime_error(std::string("gemm_reduce_scatter launch: ") + cudaGetErrorString(e));
   }, py::arg("accl"), py::arg("a_ptr"), py::arg("w_ptr"), py::arg("out"), py::arg("M"), py::arg("N"), py::arg("K"), py::arg("stream"),
         py::arg("variant") = 0, py::arg("status_dev_ptr") = 0, py::arg("w_kn") = false, py::call_guard<py::gil_scoped_release>());
+  // out[M, N] (heap buffer, bf16 or fp32, the same on every rank) = allreduce( A[M,K] @ W[N,K]^T ) (or @ W[K,N] with
+  // w_kn), fused on wgmma + NVLink; counters: the heap block of GEMM_AR_MAX_TILES uint32 words the kernel signals in
+  m.attr("gemm_ar_max_tiles") = GEMM_AR_MAX_TILES;
+  m.def("gemm_all_reduce", [](ACCL &a, uintptr_t a_ptr, uintptr_t w_ptr, BaseBuffer &out, BaseBuffer &counters, uint32_t M, uint32_t N,
+                              uint32_t K, uintptr_t stream, int variant, uintptr_t status_dev_ptr, bool w_kn) {
+    auto *d = dynamic_cast<CudaDevice *>(a.device());
+    if (!d) throw std::runtime_error("not a CUDA backend");
+    GemmArArgs g{reinterpret_cast<const void *>(a_ptr), reinterpret_cast<const void *>(w_ptr), out.address(), counters.address(), M, N, K};
+    g.variant = variant;
+    g.out_f32 = out.type() == dataType::float32;
+    g.status_dev = reinterpret_cast<uint32_t *>(status_dev_ptr);
+    g.w_kn = w_kn;
+    if (!g.out_f32 && out.type() != dataType::bfloat16) throw std::invalid_argument("gemm_all_reduce: C must be bf16 or fp32");
+    cudaError_t e = launch_gemm_ar(*d, g, reinterpret_cast<cudaStream_t>(stream));
+    if (e != cudaSuccess) throw std::runtime_error(std::string("gemm_all_reduce launch: ") + cudaGetErrorString(e));
+  }, py::arg("accl"), py::arg("a_ptr"), py::arg("w_ptr"), py::arg("out"), py::arg("counters"), py::arg("M"), py::arg("N"), py::arg("K"),
+        py::arg("stream"), py::arg("variant") = 0, py::arg("status_dev_ptr") = 0, py::arg("w_kn") = false,
+        py::call_guard<py::gil_scoped_release>());
   // out[M, N] = allgather_M(shard[M/P, K]) @ W[N, K]^T (or @ W[K, N] with w_kn), fused on wgmma + NVLink; gathered[M, K]
   // receives the gathered rows
   m.def("all_gather_gemm", [](ACCL &a, BaseBuffer &shard, uintptr_t w_ptr, uintptr_t gathered_ptr, uintptr_t out_ptr, uint32_t M,

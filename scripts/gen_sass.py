@@ -35,12 +35,12 @@ EXCERPTS = [
     ("persistent engine: command fetch / parked-call loop of the control CTA", "k_engine", r"NANOSLEEP", 20, 20,
      "the control CTA polls the command ring with `ld.acquire.sys`, steps every call in flight and backs off with NANOSLEEP "
      "only after 100 us without work."),
-    ("wgmma GEMM: MMA issue loop", "k_plugin_gemm_rs_true_false_false", r"HGMMA\.64x256x16", 6, 30,
+    ("wgmma GEMM: MMA issue loop", "k_plugin_gemm_rs_true_false_false_false", r"HGMMA\.64x256x16", 6, 30,
      "`wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16` from shared-memory descriptors, issued by each consumer "
      "warpgroup into its register accumulators."),
-    ("wgmma GEMM, CTA pair: TMA loads", "k_plugin_gemm_rs_true_false_false", r"UTMALDG\.2D\.MULTICAST", 4, 10,
+    ("wgmma GEMM, CTA pair: TMA loads", "k_plugin_gemm_rs_true_false_false_false", r"UTMALDG\.2D\.MULTICAST", 4, 10,
      "`cp.async.bulk.tensor.2d ... multicast::cluster`: each CTA of the pair loads half of the W tile into both CTAs."),
-    ("wgmma GEMM epilogue: registers -> swizzled smem -> TMA reduce-add into the owner rank's shard", "k_plugin_gemm_rs_true_false_false",
+    ("wgmma GEMM epilogue: registers -> swizzled smem -> TMA reduce-add into the owner rank's shard", "k_plugin_gemm_rs_true_false_false_false",
      r"UTMAREDG\.2D\.ADD", 30, 6,
      "`UTMAREDG.2D.ADD` = `cp.reduce.async.bulk.tensor.2d ... .add`: the tile is added into "
      "peer memory over NVLink by the TMA unit (device API `reduce_scatter_emit_tile`)."),
@@ -54,7 +54,17 @@ EXCERPTS = [
      r"UTMASTG\.2D", 30, 6,
      "`UTMASTG.2D` = `cp.async.bulk.tensor.2d.global.shared::cta.bulk_group`: the bf16 tile leaves shared memory for the "
      "local C through the TMA unit."),
-    ("wgmma GEMM with a [K, N] weight: MMA issue loop", "k_plugin_gemm_rs_true_false_true", r"HGMMA\.64x256x16", 6, 30,
+    ("GEMM -> all-reduce: lazy per-tile signal to the owner", "k_plugin_gemm_rs_true_false_false_true", r"DEPBAR\.LE SB0, 0x0", 4, 40,
+     "at the next tile's epilogue a consumer warp's lane 0 waits for its previous tile's reduce-adds to be performed "
+     "(`cp.async.bulk.wait_group 0` = `DEPBAR.LE SB0, 0x0`), orders them before its generic accesses "
+     "(`fence.proxy.async.global` = `FENCE.VIEW.ASYNC.G`) and adds 1 to the tile's counter in the owner's heap with "
+     "`red.release.sys` (a system-scope `MEMBAR`, then `REDG.E.ADD.STRONG.SYS`)."),
+    ("GEMM -> all-reduce: the owner's broadcast of a finished tile", "k_plugin_gemm_rs_true_false_false_true",
+     r"LDG\.E\.128\.STRONG\.SYS", 4, 30,
+     "warps 1-3 of the producer warpgroup, once a tile's counter holds all P ranks' arrivals: four `ld.volatile` 16-byte "
+     "loads of the local tile in flight, then `STG.E.NA.128` stores of the same 16 bytes into every peer's C through the "
+     "peer-mapped heap."),
+    ("wgmma GEMM with a [K, N] weight: MMA issue loop", "k_plugin_gemm_rs_true_false_true_false", r"HGMMA\.64x256x16", 6, 30,
      "the same instruction with `.tnspB`: B is read MN-major from 64-column boxes of the [K, N] weight (an nn.Linear "
      "weight in its own backward pass), the descriptor advancing 2048 bytes per K=16 step."),
 ]
