@@ -10,6 +10,9 @@
 * all_gather_gemm: the column-parallel counterpart — the GEMM starts on this
   rank's own rows while the kernel pulls the peers' shards over NVLink, and
   each peer tile waits only for its own 128 rows.
+* all_reduce_rmsnorm: the step after a row-parallel matmul with replicated
+  activations — the partial sums are all-reduced, the residual added and the
+  rows RMS-normalised in one kernel, while the reduced rows are in registers.
 * vadd_allreduce: the vector-add plugin; the kernel computes x + y chunk by
   chunk and hands every finished chunk to the persistent engine itself
   (device API, all_reduce_async) while it computes the next one.
@@ -224,6 +227,75 @@ def all_gather_gemm(accl: Accl, a_shard: torch.Tensor, w: torch.Tensor, out: tor
     _C.all_gather_gemm(accl.impl, accl.wrap_device(a_shard).impl, w.data_ptr(), gathered.data_ptr(), out.data_ptr(),
                        M, N, K, status_ptr, _stream_handle(accl), kn)
     return out, gathered
+
+
+AR_RMSNORM_MAX_H = 16384  # plugins.hpp AR_MAX_H: widest row of one all_reduce_rmsnorm call
+
+
+def all_reduce_rmsnorm(accl: Accl, x: torch.Tensor, weight: torch.Tensor, residual: torch.Tensor = None,
+                       eps: float = 1e-6, out: torch.Tensor = None, residual_out: torch.Tensor = None,
+                       status: torch.Tensor = None):
+    """All-reduce -> residual add -> RMSNorm in one kernel.  Returns (out, residual_out).
+
+        residual_out = bf16(x_0 + x_1 + ... + x_{P-1} + residual)      fp32 sum, ranks added in rank order
+        out          = bf16((residual_out * rsqrt(mean(residual_out^2) + eps)) * weight)   per row, in fp32
+
+    `x` [M, H] bf16 is this rank's partial sums (e.g. the output of a row-parallel matmul, x_r @ W_r^T), contiguous,
+    in the symmetric heap (a `Buffer.dev` view or a `heap_mem_pool()` tensor) at the same offset on every rank; it is
+    only read, and a rank may rewrite it on the stream right after the call.  `residual` [M, H] bf16 (optional) holds
+    the same values on every rank; `weight` [H] bf16 is the RMSNorm gain.  `residual_out` [M, H] bf16 must live in the
+    heap at the same offset on every rank; it is allocated when not given (the returned tensor keeps its heap buffer
+    alive) and may be `residual` itself (in-place update).  `out` [M, H] bf16 is an ordinary CUDA tensor, allocated
+    when not given.  Needs H % 8 == 0, 8 <= H <= 16384, M >= 1.  Every rank gets the same bits.
+    The sum is rounded to bf16 once, before the norm; matmul + all_reduce + add + rms_norm rounds twice (the
+    all-reduce result, then its sum with the residual), so its residual stream can differ in the last bit.
+    The kernel is one-shot (every rank pulls every row of every peer) while M H 2 P <= the "oneshot_max_bytes" tuning
+    knob, two-shot above it (each rank reduces M / P rows and pushes them into every peer's residual_out); both give
+    the same bits.  Stream ordered.
+    `status`, optional 1-element int32 CUDA tensor, receives the error bits when the kernel ends (0: success); with
+    non-zero bits the results are not valid.  An x or residual_out at a different heap offset on some peer sets
+    DMA_MISMATCH_ERROR (bit 0) on both ranks, and neither reads or writes the other's heap.
+    Raises ValueError, before anything is enqueued, for a wrong dtype, shape, device or alignment, an x or
+    residual_out outside the heap, overlapping tensors (other than residual_out being residual), or a bad eps."""
+    op = "all_reduce_rmsnorm"
+    if not isinstance(x, torch.Tensor) or not accl.heap_contains(x):
+        raise ValueError(f"{op}: x must live in the symmetric heap (a Buffer.dev view or a heap_mem_pool tensor)")
+    device = x.device
+    _check_operand(op, "x", x, device)
+    M, H = x.shape
+    if M < 1 or H % 8 or not 8 <= H <= AR_RMSNORM_MAX_H:
+        raise ValueError(f"{op}: need M >= 1, H % 8 == 0 and 8 <= H <= {AR_RMSNORM_MAX_H}; got M = {M}, H = {H}")
+    if not (isinstance(weight, torch.Tensor) and weight.device == device and weight.dtype == torch.bfloat16 and
+            tuple(weight.shape) == (H,) and weight.is_contiguous()):
+        raise ValueError(f"{op}: weight must be a contiguous bf16 tensor of shape ({H},) on {device}")
+    eps = float(eps)
+    if not (eps >= 0.0 and eps < float("inf")):
+        raise ValueError(f"{op}: eps must be finite and non-negative, got {eps}")
+    for name, t in (("residual", residual), ("residual_out", residual_out), ("out", out)):
+        if t is not None:
+            _check_operand(op, name, t, device)
+            if tuple(t.shape) != (M, H):
+                raise ValueError(f"{op}: {name} must be [{M}, {H}], got {tuple(t.shape)}")
+    if residual_out is not None and not accl.heap_contains(residual_out):
+        raise ValueError(f"{op}: residual_out must live in the symmetric heap (a Buffer.dev view or a heap_mem_pool tensor)")
+    if residual_out is not None and (_overlap(residual_out, x) or (
+            residual is not None and _overlap(residual_out, residual) and residual_out.data_ptr() != residual.data_ptr())):
+        raise ValueError(f"{op}: residual_out must not overlap x, and may overlap residual only by being the same tensor")
+    if out is not None and any(t is not None and _overlap(out, t) for t in (x, residual, residual_out, weight)):
+        raise ValueError(f"{op}: out must not overlap x, residual, residual_out or weight")
+    if any(t is not None and t.data_ptr() % 16 for t in (x, weight, residual, residual_out, out)):
+        raise ValueError(f"{op}: every tensor must start at a 16-byte aligned address")
+    status_ptr = _status_ptr(op, status, device)
+    if residual_out is None:
+        buf = accl.create_buffer(M * H, torch.bfloat16)
+        residual_out = buf.dev.view(M, H)
+        residual_out._accl_buffer = buf
+    if out is None:
+        out = torch.empty(M, H, dtype=torch.bfloat16, device=device)
+    _C.all_reduce_rmsnorm(accl.impl, accl.wrap_device(x).impl, residual.data_ptr() if residual is not None else 0,
+                          weight.data_ptr(), accl.wrap_device(residual_out).impl, out.data_ptr(), M, H, eps, status_ptr,
+                          _stream_handle(accl))
+    return out, residual_out
 
 
 def vadd_allreduce(accl: Accl, x: Buffer, y: Buffer, out: Buffer, tmp: Buffer = None, count: int = None,

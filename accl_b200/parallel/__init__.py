@@ -19,6 +19,8 @@ them on a H100 node:
 * `ReplicatedRowParallelLinear` / `ReplicatedColumnParallelLinear`  the same pair with activations replicated on every
                          rank (plain Megatron TP): the row layer's forward and the column layer's input gradient end
                          in an all-reduce that runs inside the GEMM (accl_b200.ops.gemm_all_reduce)
+* `AllReduceRMSNorm`     all-reduce of a row-parallel matmul's partial sums, residual add and RMSNorm in one kernel
+                         (accl_b200.ops.all_reduce_rmsnorm)
 * `ring_exchange`        neighbour send/recv step for context-parallel / ring-attention schedules
 * `process_group`        `torch.distributed` backend "accl" (import accl_b200.parallel.process_group): the standard
                          ProcessGroup interface incl. DistributedDataParallel on top of this library
@@ -31,7 +33,7 @@ import torch
 
 from .. import _C
 from ..core import Accl, Buffer, SUM, cuda_rank, socket_rank
-from ..ops.plugins import GEMM_AR_MAX_TILES
+from ..ops.plugins import AR_RMSNORM_MAX_H, GEMM_AR_MAX_TILES
 from ..utils.dtypes import to_accl
 
 
@@ -655,6 +657,108 @@ class ReplicatedColumnParallelLinear(torch.nn.Module):
             return _ReplicatedColumnFn.apply(x, self.weight, self)
         with torch.no_grad():
             return x @ self.weight.t()
+
+
+def ar_rmsnorm_fused(cuda, comm_id, dtype, m, hidden):
+    """Whether AllReduceRMSNorm's forward runs on ops.all_reduce_rmsnorm: bf16 rows of 8 to 16384 features, a multiple
+    of 8, on the world communicator of the CUDA backend."""
+    return (cuda and comm_id == 0 and dtype == torch.bfloat16 and m >= 1 and hidden % 8 == 0 and
+            8 <= hidden <= AR_RMSNORM_MAX_H)
+
+
+def _rms_norm_backward(h, weight, eps, dy, dh_out):
+    """(dh, dweight) of y = rms_norm(h) * weight, from the saved h (fp32 math; rstd is recomputed)."""
+    hf = h.float()
+    rstd = torch.rsqrt(hf.pow(2).mean(-1, keepdim=True) + eps)
+    hhat = hf * rstd
+    dyf = dy.float()
+    g = dyf * weight.float()
+    dh = rstd * (g - hhat * (g * hhat).mean(-1, keepdim=True))
+    if dh_out is not None:
+        dh = dh + dh_out.float()
+    return dh, (dyf * hhat).sum(0)
+
+
+class _ArRmsNormFn(torch.autograd.Function):
+    """(y, h) = (rms_norm(h) * weight, all_reduce(partial) + residual).  y and h are replicated, so the backward is local:
+    dpartial = dresidual = dh, with dh = rstd (dy w - h^ mean(dy w h^)) + dh_out and dweight = sum_rows dy h^."""
+
+    @staticmethod
+    def forward(ctx, partial, residual, weight, layer):
+        y, h = layer._forward(partial, residual, weight, training=True)
+        ctx.eps, ctx.has_residual = layer.eps, residual is not None
+        ctx.save_for_backward(h, weight)
+        return y, h
+
+    @staticmethod
+    def backward(ctx, dy, dh_out):
+        h, weight = ctx.saved_tensors
+        dh, dw = _rms_norm_backward(h, weight, ctx.eps, dy, dh_out)
+        dh = dh.to(h.dtype)
+        return dh, (dh if ctx.has_residual else None), dw.to(weight.dtype), None
+
+
+class AllReduceRMSNorm(torch.nn.Module):
+    """(y, h) = (RMSNorm(h) * weight, all_reduce_over_ranks(partial) + residual): the step after the row-parallel matmul of
+    a transformer block whose activations are replicated on every rank.  forward(partial [m, hidden], residual=None):
+    `partial` is this rank's unreduced output of a local matmul (F.linear(x_r, W_r)), `h` the new residual stream
+    and `y` its normalisation, both replicated.
+    On the CUDA backend (bf16, hidden % 8 == 0, 8 <= hidden <= 16384, `ar_rmsnorm_fused`) the all-reduce, the residual
+    add and the norm run in one kernel (accl_b200.ops.all_reduce_rmsnorm) and every rank gets the same bits: `partial`
+    is read in place when it lives in the symmetric heap, else it is copied into a heap buffer the layer keeps, and `h`
+    is written into a second heap buffer the layer keeps.  The fused call rounds h to bf16 once; the fallback
+    (emulator, fp32, other shapes: all_reduce, add, torch rms_norm) rounds the all-reduce result and then its sum with
+    the residual.
+    Trainable: the backward is local torch math (y and h are replicated), dpartial = dresidual = dh.  With grad enabled
+    the fused call's status goes into the group's word (raised at `group.check(block=True)` / `group.barrier()`) and h is
+    copied out of the heap buffer; under no_grad / inference_mode h is a view of the heap buffer, which the layer's next
+    call rewrites (`residual=h` from the previous call is updated in place).  Every rank must build its layers and run
+    them in the same order (the heap buffers sit at the same offset on every rank)."""
+
+    def __init__(self, group: TensorGroup, hidden, eps=1e-6, dtype=torch.bfloat16, device=None):
+        super().__init__()
+        self.group = group
+        self.eps = eps
+        dev = device if device is not None else (torch.device("cuda", group.accl.cuda_device) if group.accl.is_cuda else "cpu")
+        self.weight = torch.nn.Parameter(torch.ones(hidden, dtype=dtype, device=dev))
+        self._x = None  # heap buffer of a partial that does not live in the heap
+        self._h = None  # heap buffer of the residual stream
+
+    def forward(self, partial, residual=None):
+        if torch.is_grad_enabled() and (partial.requires_grad or self.weight.requires_grad or
+                                        (residual is not None and residual.requires_grad)):
+            return _ArRmsNormFn.apply(partial, residual, self.weight, self)
+        with torch.no_grad():
+            return self._forward(partial, residual, self.weight)
+
+    def _forward(self, partial, residual, weight, training=False):
+        """training: the fused call reports into the group's status word, and h is copied out of the heap buffer."""
+        from ..ops import all_reduce_rmsnorm
+        m, n = partial.shape
+        g = self.group
+        dtype = _dtype_of(partial, weight)
+        if residual is not None and residual.dtype != dtype:
+            dtype = None
+        if ar_rmsnorm_fused(bool(g.accl.is_cuda), g.comm_id, dtype, m, n):
+            if partial.is_contiguous() and g.accl.heap_contains(partial) and partial.data_ptr() % 16 == 0:
+                x = partial
+            else:
+                x = _heap_buffer(self, "_x", m * n).dev.view(m, n)
+                x.copy_(partial)
+            h = _heap_buffer(self, "_h", m * n).dev.view(m, n)
+            res = None if residual is None else residual.detach()
+            if res is not None and not (res.is_contiguous() and res.data_ptr() % 16 == 0):
+                res = res.contiguous()
+            st = g.plugin_status() if training else None
+            y, h = all_reduce_rmsnorm(g.accl, x, weight.detach(), res, self.eps, residual_out=h, status=st)
+            if training:
+                g.note_plugin_status(st)
+                return y, h.clone()
+            return y, h
+        s = partial.detach().clone().contiguous()
+        g.all_reduce(s)
+        h = s if residual is None else s + residual.detach()
+        return torch.nn.functional.rms_norm(h, (n,), weight.detach(), self.eps), h
 
 
 def ring_exchange(group: TensorGroup, send_t: torch.Tensor, recv_t: torch.Tensor, tag=0):

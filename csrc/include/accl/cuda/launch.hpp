@@ -26,6 +26,7 @@ void preload_engine_kernels();
 void preload_gemm_rs_kernels();
 void preload_ag_gemm_kernels();
 void preload_vadd_kernels();
+void preload_ar_rmsnorm_kernels();
 
 // Device-side stream port (the user-kernel <-> engine AXI streams of the reference): a byte
 // FIFO in the heap.  pop: FIFO -> dst (local heap offset); push: src -> FIFO of rank `dst_rank`.

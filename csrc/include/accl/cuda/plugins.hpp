@@ -78,6 +78,31 @@ struct AgGemmArgs {
 // Returns after enqueueing.
 cudaError_t launch_ag_gemm(CudaDevice &dev, const AgGemmArgs &args, cudaStream_t stream);
 
+// widest row of one all-reduce -> RMSNorm call, in elements
+constexpr uint32_t AR_MAX_H = 16384;
+
+struct ArRmsNormArgs {
+  uint64_t x_off;         // heap offset of this rank's [M, H] bf16 partial sums (the same on every rank); only read
+  const void *residual;   // [M, H] bf16, the same values on every rank, or null; may be residual_out itself
+  const void *gamma;      // [H] bf16 RMSNorm gain
+  uint64_t h_off;         // heap offset of residual_out [M, H] bf16 (the same on every rank)
+  void *out;              // [M, H] bf16
+  uint32_t m, h;
+  float eps;
+  uint32_t *status_dev;   // device word that receives the error bits (0: success) when the kernel ends; may be null
+};
+
+// residual_out = bf16(sum over ranks of x_r, in rank order, + residual) and out = RMSNorm(residual_out) * gamma, in
+// one kernel: the all-reduce result is normalised while it is still in registers.  One-shot (every rank pulls every
+// row) while M H 2 P <= CudaConfig::oneshot_max_bytes, else two-shot (each rank reduces its M / P rows, pushes them
+// into every peer's residual_out, and every rank normalises all rows); both forms give the same bits.  x and
+// residual_out must sit at the same offsets on every rank: a peer where either differs is neither read nor written,
+// and the call reports DMA_MISMATCH_ERROR.  Throws std::invalid_argument before enqueueing anything unless M >= 1,
+// H % 8 == 0, 8 <= H <= AR_MAX_H, eps is finite and >= 0, both heap regions are 16-byte aligned inside the heap and
+// do not overlap, every pointer is 16-byte aligned and residual is residual_out or does not overlap it.  Returns
+// after enqueueing.
+cudaError_t launch_ar_rmsnorm(CudaDevice &dev, const ArRmsNormArgs &args, cudaStream_t stream);
+
 // vector add whose result feeds an all-reduce issued by the kernel itself through the device API (engine must be
 // enabled): out = allreduce_sum(x + y).  The vector is produced in chunks of `chunk_elems` (0: 1 Mi elements); each
 // finished chunk is handed to the engine at once (all_reduce_async) while the kernel computes the next one.

@@ -176,6 +176,20 @@ void bind_cuda(py::module_ &m) {
     if (e != cudaSuccess) throw std::runtime_error(std::string("all_gather_gemm launch: ") + cudaGetErrorString(e));
   }, py::arg("accl"), py::arg("shard"), py::arg("w_ptr"), py::arg("gathered_ptr"), py::arg("out_ptr"), py::arg("M"), py::arg("N"),
         py::arg("K"), py::arg("status_dev_ptr"), py::arg("stream"), py::arg("w_kn") = false, py::call_guard<py::gil_scoped_release>());
+  // residual_out (heap) = bf16(allreduce(x) + residual), out = RMSNorm(residual_out) * gamma, in one kernel
+  m.attr("ar_rmsnorm_max_h") = AR_MAX_H;
+  m.def("all_reduce_rmsnorm", [](ACCL &a, BaseBuffer &x, uintptr_t residual_ptr, uintptr_t gamma_ptr, BaseBuffer &residual_out,
+                                 uintptr_t out_ptr, uint32_t M, uint32_t H, float eps, uintptr_t status_dev_ptr, uintptr_t stream) {
+    auto *d = dynamic_cast<CudaDevice *>(a.device());
+    if (!d) throw std::runtime_error("not a CUDA backend");
+    if (x.type() != dataType::bfloat16 || residual_out.type() != dataType::bfloat16)
+      throw std::invalid_argument("all_reduce_rmsnorm: x and residual_out must be bf16");
+    ArRmsNormArgs g{x.address(), reinterpret_cast<const void *>(residual_ptr), reinterpret_cast<const void *>(gamma_ptr),
+                    residual_out.address(), reinterpret_cast<void *>(out_ptr), M, H, eps, reinterpret_cast<uint32_t *>(status_dev_ptr)};
+    cudaError_t e = launch_ar_rmsnorm(*d, g, reinterpret_cast<cudaStream_t>(stream));
+    if (e != cudaSuccess) throw std::runtime_error(std::string("all_reduce_rmsnorm launch: ") + cudaGetErrorString(e));
+  }, py::arg("accl"), py::arg("x"), py::arg("residual_ptr"), py::arg("gamma_ptr"), py::arg("residual_out"), py::arg("out_ptr"),
+        py::arg("M"), py::arg("H"), py::arg("eps"), py::arg("status_dev_ptr"), py::arg("stream"), py::call_guard<py::gil_scoped_release>());
   // out = allreduce_sum(x + y): the kernel computes and then issues the collective itself (device API -> engine)
   m.def("vadd_allreduce", [](ACCL &a, BaseBuffer &x, BaseBuffer &y, BaseBuffer &tmp, BaseBuffer &out, uint32_t count,
                              uintptr_t status_dev_ptr, uintptr_t stream, uint32_t chunk_elems) {

@@ -258,6 +258,7 @@ CudaDevice::CudaDevice(std::shared_ptr<Oob> oob, const CudaConfig &cfg) : oob_(s
   preload_gemm_rs_kernels();
   preload_ag_gemm_kernels();
   preload_vadd_kernels();
+  preload_ar_rmsnorm_kernels();
   (void)plugin_scratch(16u << 10); // allocate now: cudaMalloc later could stall behind a running engine kernel
   ACCL_CUDART(launch_reset_ctrl(world_, stream_));
   ACCL_CUDART(cudaStreamSynchronize(stream_));
