@@ -28,6 +28,12 @@ void preload_ag_gemm_kernels();
 void preload_vadd_kernels();
 void preload_ar_rmsnorm_kernels();
 
+class CudaDevice;
+// The flag block of fused plugin `plugin` on `dev` (layout: PluginFlag, kernels.cuh): `words` uint32 words of device
+// memory, allocated at the first call and zeroed on `stream` at every call, so each launch finds it zeroed and the
+// launch can be captured in a CUDA graph.  Each plugin passes its own tag and the same `words` every time.
+unsigned int *plugin_flags(CudaDevice &dev, char plugin, uint32_t words, cudaStream_t stream);
+
 // Device-side stream port (the user-kernel <-> engine AXI streams of the reference): a byte
 // FIFO in the heap.  pop: FIFO -> dst (local heap offset); push: src -> FIFO of rank `dst_rank`.
 cudaError_t launch_stream_pop(const DevWorld &w, uint64_t dst_off, uint64_t bytes, uint32_t stream_id, uint32_t timeout_us,

@@ -18,7 +18,6 @@ struct GemmRsArgs {
   const void *w;     // [N, K] bf16 row-major (this rank's K-slice of the weight, nn.Linear layout), or [K, N] with w_kn
   uint64_t out_off;  // heap offset of this rank's [M / P, N] output shard (bf16, or fp32 with out_f32)
   uint32_t m, n, k;
-  uint32_t epoch;    // launch counter (same on every rank), starts at 1
   int variant = 0;   // 0: automatic, 1: one CTA per 128 x 256 tile, 2: CTA pair (cluster of 2, W tile multicast) per 256 x 256 tile
   bool out_f32 = false; // shard is fp32: the P partial products are added without intermediate rounding
   uint32_t *status_dev = nullptr; // device word that receives the error bits (0: success) when the kernel ends; may be null

@@ -135,7 +135,7 @@ void bind_cuda(py::module_ &m) {
                                   uintptr_t stream, int variant, uintptr_t status_dev_ptr, bool w_kn) {
     auto *d = dynamic_cast<CudaDevice *>(a.device());
     if (!d) throw std::runtime_error("not a CUDA backend");
-    GemmRsArgs g{reinterpret_cast<const void *>(a_ptr), reinterpret_cast<const void *>(w_ptr), out.address(), M, N, K, 0};
+    GemmRsArgs g{reinterpret_cast<const void *>(a_ptr), reinterpret_cast<const void *>(w_ptr), out.address(), M, N, K};
     g.variant = variant;
     g.out_f32 = out.type() == dataType::float32;
     g.status_dev = reinterpret_cast<uint32_t *>(status_dev_ptr);

@@ -129,6 +129,26 @@ private:
 };
 } // namespace
 
+unsigned int *plugin_flags(CudaDevice &dev, char plugin, uint32_t words, cudaStream_t stream) {
+  static std::mutex m;
+  static std::map<std::pair<CudaDevice *, char>, unsigned int *> blocks;
+  unsigned int *f;
+  {
+    std::lock_guard<std::mutex> lk(m);
+    unsigned int *&b = blocks[{&dev, plugin}];
+    if (!b) {
+      // the blocking memset is not redundant with the one on the stream below: without it the first launch on a new
+      // device can start waiting for its peers while a rank sharing this GPU is still inside a device-synchronising
+      // call of its own set-up, and both ranks sit out the call timeout
+      ACCL_CUDART(cudaMalloc(&b, words * sizeof(unsigned int)));
+      ACCL_CUDART(cudaMemset(b, 0, words * sizeof(unsigned int)));
+    }
+    f = b;
+  }
+  ACCL_CUDART(cudaMemsetAsync(f, 0, words * sizeof(unsigned int), stream));
+  return f;
+}
+
 // ------------------------------------------------------------------ request
 CudaRequest::~CudaRequest() {}
 

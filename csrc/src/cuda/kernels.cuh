@@ -73,8 +73,8 @@ __device__ __forceinline__ bool wait_ge(const uint32_t *p, uint32_t target, cons
 // A meeting of this rank with one peer on channel `ch` of the call's bank (global rank `peer`): each side posts
 // (sent += 1, optionally a record, then the release of the peer's `sig`), then takes the peer's post (expect += 1)
 // once `sig` has reached it.  The pad layout and the record format are known only to the helpers below.  They are
-// per thread and never call __syncthreads: a CTA serves its peers with one thread each, the GEMM plugin with one lane
-// each, and the engine polls with `pad_arrived` instead of blocking.
+// per thread and never call __syncthreads: a CTA serves its peers with one thread each, the fused plugins one lane each
+// (meet_peers, below), and the engine polls with `pad_arrived` instead of blocking.
 
 // which fields of the record a post carries: none (a bare signal), off0 + kind, or off0 + off2 + kind
 enum PadRec : uint32_t { REC_NONE, REC_OFF0, REC_OFFS };
@@ -173,6 +173,87 @@ __device__ __forceinline__ void pair_sync(const Ctx &c, uint32_t peer_comm_rank,
     }
   }
   __syncthreads();
+}
+
+// ------------------------------------------------ fused plugin kernels
+// The fused plugins (plugin_gemm_rs.cu, plugin_ag_gemm.cu, plugin_ar_rmsnorm.cu) meet their peers on the sync pads of
+// channel MAX_CH-1, bank 0, through an identity communicator whose kind word names the plugin, and coordinate their
+// grid through a flag block in device memory that the host zeroes on the stream before every launch
+// (plugin_flags, launch.hpp).  Words of the block; a plugin's own words start at FLAG_PLUGIN.
+enum PluginFlag : uint32_t {
+  FLAG_RELEASE, // the entry meeting is over: FLAG_MASK is valid
+  FLAG_DONE,    // CTAs that have finished
+  FLAG_ERR,     // error bits of the grid
+  FLAG_MASK,    // meet_peers' mask
+  FLAG_PLUGIN
+};
+
+// The identity communicator of a plugin kernel (world ranks, channel MAX_CH-1 of bank 0).  scenario and comm_sig make
+// up its kind word: a peer inside another plugin reports PACK_SEQ_NUMBER_ERROR.
+__device__ __forceinline__ void plugin_item(WorkItem &it, const DevWorld &w, uint32_t scenario, uint32_t comm_sig, uint32_t timeout_us) {
+  it.comm_size = w.world;
+  it.comm_rank = w.rank;
+  for (uint32_t r = 0; r < static_cast<uint32_t>(ACCL_MAX_RANKS); ++r) it.members[r] = static_cast<uint8_t>(r < w.world ? r : 0);
+  it.desc.scenario = scenario;
+  it.timeout_us = timeout_us;
+  it.bank = 0;
+  it.comm_sig = comm_sig;
+}
+
+// Entry meeting of a plugin kernel, called by one whole warp: lane q meets rank q on channel MAX_CH-1 and posts
+// (off0, off2) with `rec` (REC_OFF0: off0 only).  Returns the ranks whose post carries this kernel's kind word and the
+// same offsets; this rank's bit is always set.  A peer in another plugin sets PACK_SEQ_NUMBER_ERROR, one whose offsets
+// differ DMA_MISMATCH_ERROR, one that does not answer within the call timeout RECEIVE_TIMEOUT_ERROR.
+__device__ __forceinline__ uint32_t meet_peers(const Ctx &c, PadRec rec, uint64_t off0, uint64_t off2) {
+  const uint32_t lane = threadIdx.x % 32, ch = MAX_CH - 1;
+  bool ok = lane == c.w.rank;
+  if (lane < c.w.world && lane != c.w.rank) {
+    pad_post(c, ch, lane, rec, off0, off2, c.kind_word());
+    if (pad_wait(c, ch, lane)) {
+      const SyncRec r = pad_rec(c, ch, lane, rec);
+      if (r.kind != c.kind_word())
+        atomicOr(c.err, PACK_SEQ_NUMBER_ERROR);
+      else if (r.off0 != off0 || (rec == REC_OFFS && r.off2 != off2))
+        atomicOr(c.err, DMA_MISMATCH_ERROR);
+      else
+        ok = true;
+    }
+  }
+  return __ballot_sync(0xffffffffu, ok);
+}
+
+// Release the grid after the entry meeting (one thread): publish the mask of meet_peers, then the release.
+__device__ __forceinline__ void release_grid(unsigned int *flags, uint32_t mask) {
+  flags[FLAG_MASK] = mask;
+  __threadfence();
+  st_release_gpu(&flags[FLAG_RELEASE], 1u);
+}
+
+// Wait for release_grid (one thread) and return its mask; on timeout RECEIVE_TIMEOUT_ERROR and this rank alone.
+__device__ __forceinline__ uint32_t wait_grid(const unsigned int *flags, const Ctx &c) {
+  const bool released = wait_ge(&flags[FLAG_RELEASE], 1u, c, RECEIVE_TIMEOUT_ERROR);
+  return (released ? *reinterpret_cast<const volatile unsigned int *>(&flags[FLAG_MASK]) : 0u) | (1u << c.w.rank);
+}
+
+// Exit of a plugin kernel, called by every thread of every CTA once the CTA's work is done: OR the CTA's error bits
+// into the block and count the CTA finished.  The last CTA of the grid meets every peer once more when `meet` (so no
+// rank rewrites what a peer still reads, or leaves while a peer still writes into it) and publishes the error bits of
+// the grid to `status` (0: success; may be null).  s_last: a shared word of the CTA, declared with its other shared
+// words (a shared variable of its own here moves the kernel's shared layout, which cost the RMSNorm kernel a register).
+__device__ __forceinline__ void plugin_exit(const Ctx &c, unsigned int *flags, uint32_t *status, bool meet, uint32_t &s_last) {
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    if (*c.err) atomicOr(&flags[FLAG_ERR], *c.err);
+    // GPU scope suffices: every write into a peer is followed by __threadfence_system() in the thread that made it,
+    // before the CTA gets here.  A system-scope fence here cost the RMSNorm kernel ~2 us a call on an H100.
+    __threadfence(); // this CTA's writes are performed before it counts itself finished
+    s_last = atomicAdd(&flags[FLAG_DONE], 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  if (meet) chan_sync(c, false, 0, 0, nullptr, nullptr);
+  if (threadIdx.x == 0 && status) *status = atomicOr(&flags[FLAG_ERR], *c.err) | *c.err;
 }
 
 // ------------------------------------------------------ exchange patterns

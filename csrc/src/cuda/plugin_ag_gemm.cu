@@ -22,15 +22,16 @@
 // Meetings on the sync pads of channel MAX_CH-1: at entry CTA 0 exchanges the shard offsets with every peer (one lane
 // per peer) and releases the copy warps of the grid; at exit the last CTA to finish meets the peers again, so no rank
 // writes its shard on its stream before every peer has read it.
+// The pipeline and the epilogue live in wgmma.cuh; the entry meeting, the grid release and the exit in kernels.cuh.
+// This file keeps the pull, the tile order and its ready[] waits, and the host launch code.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
 #include <algorithm>
-#include <map>
-#include <mutex>
 
 #include "accl/cuda/cudadevice.hpp"
 #include "accl/cuda/driver_api.hpp"
+#include "accl/cuda/launch.hpp"
 #include "accl/cuda/plugins.hpp"
 #include "accl/device/api.cuh"
 #include "kernels.cuh"
@@ -41,9 +42,8 @@ namespace cuda {
 
 namespace {
 constexpr uint32_t AG_MAX_ROW_BLOCKS = 1024; // M / 128 of one call
-// flag words, zeroed before every launch: [0] release of the copy warps, [1] finished CTAs, [2] error bits,
-// [8, 8 + 2P) the peers' shard offsets (uint64), [AG_READY, AG_READY + M/128) ready[row block]: CTAs that have copied
-// their slice of those 128 rows into `gathered`
+// flag block (kernels.cuh, PluginFlag); own words: [AG_READY, AG_READY + M/128) ready[row block], the CTAs that have
+// copied their slice of those 128 rows into `gathered`
 constexpr uint32_t AG_READY = 64;
 constexpr uint32_t AG_FLAG_WORDS = AG_READY + AG_MAX_ROW_BLOCKS;
 constexpr int COPY_THREADS = 96; // warps 1-3
@@ -58,31 +58,6 @@ struct AgGemmParams {
   unsigned int *flags;
   uint32_t *status;
 };
-
-// one 16 x 64 bf16 box of staged shared memory -> C by the TMA unit (a bulk group of this thread)
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap *map, const void *smem_src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(map)),
-               "r"(g::smem_u32(smem_src)), "r"(c0), "r"(c1)
-               : "memory");
-  asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-}
-
-template <int C>
-__device__ __forceinline__ void store_chunks(const float (&d)[128], uint8_t *my_epi, uint32_t &ebuf, int lane, const CUtensorMap *map,
-                                             int col0, int row) {
-  if constexpr (C < g::BN / 64) {
-    uint8_t *buf = my_epi + ebuf * g::EPI_BUF_BYTES;
-    // the TMA unit must be done READING this buffer (stored two chunks ago)
-    if (lane == 0) device::emit_wait_read<1>();
-    __syncwarp();
-    epilogue_chunk<false, C>(d, buf, lane);
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); // generic-proxy writes -> visible to the TMA unit
-    __syncwarp();
-    if (lane == 0) tma_store_2d(map, buf, col0 + C * 64, row);
-    ebuf ^= 1;
-    store_chunks<C + 1>(d, my_epi, ebuf, lane, map, col0, row);
-  }
-}
 
 // this thread's share of one chunk: 16-byte vectors i, i + stride, ...; four loads in flight before their stores
 __device__ __forceinline__ void copy_slice(const char *src, char *dst, size_t nvec, size_t i, size_t stride) {
@@ -106,13 +81,6 @@ k_plugin_ag_gemm(const __grid_constant__ CUtensorMap tmap_own, const __grid_cons
   using namespace g;
   constexpr int GROUP_M = 16;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint8_t *smem_a = smem;
-  uint8_t *smem_b = smem + STAGES * A_STAGE_BYTES;
-  uint8_t *smem_epi = smem + STAGES * STAGE_BYTES;
-  uint64_t *bars = reinterpret_cast<uint64_t *>(smem + STAGES * STAGE_BYTES + EPI_BYTES);
-  uint64_t *full = bars, *empty = bars + STAGES;
-
   __shared__ uint32_t s_err, s_readable, s_last;
   __shared__ WorkItem s_item; // identity communicator for the sync pads
 
@@ -123,24 +91,12 @@ k_plugin_ag_gemm(const __grid_constant__ CUtensorMap tmap_own, const __grid_cons
   const uint32_t blocks_per_rank = tiles_m / P; // 128-row chunks of one shard
   char *my_heap = p.w.window + static_cast<uint64_t>(me) * p.w.heap_bytes;
   unsigned int *ready = p.flags + AG_READY;
-  volatile uint64_t *peer_off = reinterpret_cast<volatile uint64_t *>(p.flags + 8);
 
   // ---------------- one-time setup
+  const Smem sm = gemm_smem<false>(smem_raw);
   if (threadIdx.x == 0) {
     s_err = 0;
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full[i], 1);  // the producer's arrive.expect_tx
-      mbar_init(&empty[i], 2); // one arrival per consumer warpgroup
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    s_item.comm_size = P;
-    s_item.comm_rank = me;
-    for (uint32_t r = 0; r < static_cast<uint32_t>(ACCL_MAX_RANKS); ++r) s_item.members[r] = static_cast<uint8_t>(r < P ? r : 0);
-    s_item.desc.scenario = 0x41; // 'A': both ends must be in this plugin (GEMM -> reduce-scatter uses 'G')
-    s_item.timeout_us = p.timeout_us;
-    s_item.bank = 0;
-    s_item.comm_sig = 0x414747u;
+    k::plugin_item(s_item, p.w, 0x41, 0x414747u, p.timeout_us); // 'A'
   }
   if (warp == 0 && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_own)) : "memory");
@@ -156,34 +112,12 @@ k_plugin_ag_gemm(const __grid_constant__ CUtensorMap tmap_own, const __grid_cons
     // ===== pull the shards into `gathered`
     if (blockIdx.x == 0 && warp == 1) {
       // entry meeting with every peer, one lane each: exchange the shard offsets.  A peer that does not answer, is in
-      // another operation or has its shard elsewhere is not read (INVALID_OFF).
-      uint64_t off = p.a_off;
-      if (static_cast<uint32_t>(lane) < P && static_cast<uint32_t>(lane) != me) {
-        k::pad_post(ctx, MAX_CH - 1, lane, k::REC_OFF0, p.a_off, 0, ctx.kind_word());
-        off = INVALID_OFF;
-        if (k::pad_wait(ctx, MAX_CH - 1, lane)) {
-          const SyncRec r = k::pad_rec(ctx, MAX_CH - 1, lane, k::REC_OFF0);
-          if (r.kind != ctx.kind_word()) {
-            atomicOr(&s_err, PACK_SEQ_NUMBER_ERROR);
-          } else {
-            off = r.off0;
-            if (off != p.a_off) atomicOr(&s_err, DMA_MISMATCH_ERROR);
-          }
-        }
-      }
-      if (static_cast<uint32_t>(lane) < P) peer_off[lane] = off;
-      __threadfence();
-      __syncwarp();
-      if (lane == 0) dev::st_release_gpu(&p.flags[0], 1u); // release the copy warps of every CTA
+      // another operation or has its shard elsewhere is not read.
+      const uint32_t mask = k::meet_peers(ctx, k::REC_OFF0, p.a_off, 0);
+      if (lane == 0) k::release_grid(p.flags, mask); // release the copy warps of every CTA
     }
     const uint32_t ct = threadIdx.x - 32;
-    if (ct == 0) {
-      uint32_t readable = 1u << me;
-      if (k::wait_ge(&p.flags[0], 1u, ctx, RECEIVE_TIMEOUT_ERROR))
-        for (uint32_t q = 0; q < P; ++q)
-          if (peer_off[q] == p.a_off) readable |= 1u << q;
-      s_readable = readable;
-    }
+    if (ct == 0) s_readable = k::wait_grid(p.flags, ctx);
     asm volatile("bar.sync 1, 96;" ::: "memory"); // warps 1-3 only
     const uint32_t readable = s_readable;
     const size_t chunk_bytes = static_cast<size_t>(BM) * p.k * 2;
@@ -216,36 +150,14 @@ k_plugin_ag_gemm(const __grid_constant__ CUtensorMap tmap_own, const __grid_cons
         asm volatile("fence.proxy.async.global;" ::: "memory");
       }
       __syncwarp();
-      const CUtensorMap *map_a = own ? &tmap_own : &tmap_gathered;
-      const int row_a = static_cast<int>((own ? mo : mb) * BM);
-      for (uint32_t kb = 0; kb < k_blocks; ++kb) {
-        if (lane == 0) {
-          mbar_wait(&empty[stage], phase ^ 1);
-          mbar_expect_tx(&full[stage], STAGE_BYTES);
-          tma_load_2d(smem_a + stage * A_STAGE_BYTES, map_a, &full[stage], static_cast<int>(kb * BK), row_a);
-          if constexpr (KN) {
-            // W is [K, N]: boxes of 64 columns x 64 K-rows, one 8 KB column of swizzle atoms each
-#pragma unroll
-            for (int j = 0; j < BN / 64; ++j)
-              tma_load_2d(smem_b + stage * B_STAGE_BYTES + j * (64 * BK * 2), &tmap_w, &full[stage], static_cast<int>(nb * BN + 64 * j),
-                          static_cast<int>(kb * BK));
-          } else {
-            tma_load_2d(smem_b + stage * B_STAGE_BYTES, &tmap_w, &full[stage], static_cast<int>(kb * BK), static_cast<int>(nb * BN));
-          }
-        }
-        __syncwarp();
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
+      produce_tile<false, KN>(sm, own ? &tmap_own : &tmap_gathered, static_cast<int>((own ? mo : mb) * BM), &tmap_w, nb, k_blocks, 0,
+                              stage, phase, lane);
     }
   } else {
     // ===== consumers: wgmma into registers, then registers -> bf16 -> swizzled smem -> TMA store into C
     const uint32_t wg = warp / 4 - 1; // rows [64 wg, 64 wg + 64) of the CTA's 128
     const uint32_t wi = warp % 4;     // this warp's 16 of them
-    const bool signaller = threadIdx.x % 128 == 0;
-    uint8_t *my_epi = smem_epi + (warp - 4) * 2 * EPI_BUF_BYTES;
+    uint8_t *my_epi = sm.epi + (warp - 4) * 2 * EPI_BUF_BYTES;
     uint32_t stage = 0, phase = 0, ebuf = 0;
     float d[128];
 #pragma unroll
@@ -254,57 +166,21 @@ k_plugin_ag_gemm(const __grid_constant__ CUtensorMap tmap_own, const __grid_cons
       uint32_t mo, nb;
       tile_coords<GROUP_M>(t, tiles_m, tiles_n, mo, nb);
       const uint32_t mb = (mo + me * blocks_per_rank) % tiles_m;
-      uint32_t prev = 0;
-      for (uint32_t kb = 0; kb < k_blocks; ++kb) {
-        mbar_wait(&full[stage], phase);
-        const uint64_t da = make_smem_desc(smem_u32(smem_a + stage * A_STAGE_BYTES + wg * 64 * 128));
-        const uint32_t b_addr = smem_u32(smem_b + stage * B_STAGE_BYTES);
-        const uint64_t db = KN ? make_smem_desc_mn(b_addr) : make_smem_desc(b_addr);
-        constexpr uint64_t DB_STEP = KN ? 128 : 2; // per K=16 step, >> 4: 16 K-rows of 128 B (MN-major), 32 B (K-major)
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < BK / WGMMA_K; ++kk) // A: +32 bytes (>>4 = 2) per K=16 step inside the swizzle atom
-          wgmma_m64n256k16<KN ? 1 : 0>(d, da + 2 * kk, db + DB_STEP * kk, (kb | kk) ? 1u : 0u);
-        wgmma_commit();
-        wgmma_wait<1>(); // the previous stage's MMAs have retired: it may be refilled
-        if (kb > 0 && signaller) mbar_arrive(&empty[prev]);
-        prev = stage;
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-      wgmma_wait<0>();
-      if (signaller) mbar_arrive(&empty[prev]);
+      consume_tile<false, KN>(sm, d, wg, k_blocks, 0, stage, phase);
       const uint32_t row0 = mb * BM + wg * 64 + wi * EPI_ROWS; // first of this warp's 16 rows of C
-      store_chunks<0>(d, my_epi, ebuf, lane, &tmap_c, static_cast<int>(nb * BN), static_cast<int>(row0));
+      epilogue_tile<false, false>(d, my_epi, ebuf, lane, &tmap_c, static_cast<int>(nb * BN), static_cast<int>(row0));
     }
     if (lane == 0) device::emit_flush(); // all my stores have been written
     __syncwarp();
   }
 
   // ---------------- teardown: a CTA has finished once its copies and its tiles are done; the last one meets the peers
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    if (s_err) atomicOr(&p.flags[2], s_err);
-    __threadfence();
-    s_last = atomicAdd(&p.flags[1], 1u) == G - 1 ? 1u : 0u;
-  }
-  __syncthreads();
-  if (s_last) {
-    __threadfence();
-    // every CTA of this rank has read what it needed of the peers' shards: when all ranks meet here, each may overwrite its shard
-    k::chan_sync(ctx, false, 0, 0, nullptr, nullptr);
-    if (threadIdx.x == 0 && p.status) *p.status = atomicOr(&p.flags[2], s_err) | s_err;
-  }
+  // (every CTA of this rank has read what it needed of the peers' shards: when all ranks meet there, each may
+  // overwrite its shard)
+  k::plugin_exit(ctx, p.flags, p.status, true, s_last);
 }
 
 // ----------------------------------------------------------------------- host
-namespace {
-std::mutex g_ag_m;
-std::map<CudaDevice *, unsigned int *> g_ag_flags;
-} // namespace
-
 void preload_ag_gemm_kernels() {
   cudaFuncAttributes a;
   cudaFuncGetAttributes(&a, k_plugin_ag_gemm<false>);
@@ -326,16 +202,6 @@ cudaError_t launch_ag_gemm(CudaDevice &dev, const AgGemmArgs &a, cudaStream_t st
   if (a.a_off + static_cast<uint64_t>(a.m / P) * a.k * 2 > w.heap_bytes)
     throw std::invalid_argument("ag_gemm: the shard does not fit in the symmetric heap at that offset");
   ACCL_CUDART(cudaSetDevice(dev.device()));
-  unsigned int *flags;
-  {
-    std::lock_guard<std::mutex> lk(g_ag_m);
-    unsigned int *&f = g_ag_flags[&dev];
-    if (!f) {
-      ACCL_CUDART(cudaMalloc(&f, AG_FLAG_WORDS * sizeof(unsigned int)));
-      ACCL_CUDART(cudaMemset(f, 0, AG_FLAG_WORDS * sizeof(unsigned int)));
-    }
-    flags = f;
-  }
   const CUtensorMap t_own = make_map(w.window + static_cast<uint64_t>(w.rank) * w.heap_bytes + a.a_off, a.m / P, a.k, BM, BK);
   const CUtensorMap t_gathered = make_map(a.gathered, a.m, a.k, BM, BK);
   const CUtensorMap t_w = a.w_kn ? make_map(a.w, a.k, a.n, BK, 64) : make_map(a.w, a.n, a.k, BN, BK);
@@ -348,11 +214,10 @@ cudaError_t launch_ag_gemm(CudaDevice &dev, const AgGemmArgs &a, cudaStream_t st
   p.n = a.n;
   p.k = a.k;
   p.timeout_us = dev.timeout_us();
-  p.flags = flags;
+  p.flags = plugin_flags(dev, 'A', AG_FLAG_WORDS, stream);
   p.status = a.status_dev;
   int sms = 0;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev.device());
-  ACCL_CUDART(cudaMemsetAsync(flags, 0, AG_FLAG_WORDS * sizeof(unsigned int), stream));
   const uint32_t tiles = (a.m / BM) * (a.n / BN);
   const auto kernel = a.w_kn ? k_plugin_ag_gemm<true> : k_plugin_ag_gemm<false>;
   cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);

@@ -24,15 +24,15 @@
 // word 'N' / "ARN": the entry meeting exchanges the offsets of x and residual_out.  A peer in another plugin reports
 // PACK_SEQ_NUMBER_ERROR; a peer where either offset differs is neither read nor written, and both report
 // DMA_MISMATCH_ERROR.  The result is released to the grid through flags in device memory zeroed before the launch.
+// The identity communicator, the grid release, the exit and the flag layout are the other fused plugins' (kernels.cuh).
 #include <cuda_bf16.h>
 
 #include <algorithm>
 #include <cmath>
-#include <map>
-#include <mutex>
 
 #include "accl/cuda/cudadevice.hpp"
 #include "accl/cuda/driver_api.hpp"
+#include "accl/cuda/launch.hpp"
 #include "accl/cuda/plugins.hpp"
 #include "kernels.cuh"
 
@@ -43,9 +43,8 @@ namespace {
 constexpr int AR_THREADS = 512;
 constexpr int AR_VPT = AR_MAX_H / 8 / AR_THREADS; // 16-byte vectors of a row per thread
 static_assert(AR_VPT * 8 * AR_THREADS == static_cast<int>(AR_MAX_H), "a row of AR_MAX_H elements fills the block");
-// flag words, zeroed before every launch: [0] entry release, [1] phase-1 arrivals (two-shot), [2] middle release
-// (two-shot), [3] finished CTAs, [4] error bits, [5] peers whose offsets match (bit per rank)
-constexpr uint32_t AR_FLAG_WORDS = 8;
+// flag block (kernels.cuh, PluginFlag); own words of the two-shot form: CTAs done with phase 1, and the middle release
+constexpr uint32_t AR_PHASE1 = k::FLAG_PLUGIN, AR_MIDDLE = AR_PHASE1 + 1, AR_FLAG_WORDS = AR_MIDDLE + 1;
 } // namespace
 
 struct ArRmsNormParams {
@@ -181,18 +180,14 @@ __global__ void __launch_bounds__(AR_THREADS, 1) k_plugin_ar_rmsnorm(ArRmsNormPa
 
   if (threadIdx.x == 0) {
     s_err = 0;
-    s_item.comm_size = P;
-    s_item.comm_rank = me;
-    for (uint32_t r = 0; r < static_cast<uint32_t>(ACCL_MAX_RANKS); ++r) s_item.members[r] = static_cast<uint8_t>(r < P ? r : 0);
-    s_item.desc.scenario = 0x4E; // 'N': both ends must be in this plugin (the GEMM plugins use 'A', 'G' and 'R')
-    s_item.timeout_us = p.timeout_us;
-    s_item.bank = 0;
-    s_item.comm_sig = 0x41524Eu;
+    k::plugin_item(s_item, p.w, 0x4E, 0x41524Eu, p.timeout_us); // 'N' (the GEMM plugins use 'A', 'G' and 'R')
   }
   __syncthreads();
   k::Ctx ctx{p.w, s_item, MAX_CH - 1, 1, reinterpret_cast<Ctrl *>(my_heap), &s_err, static_cast<uint64_t>(p.timeout_us) * 1000ull, nullptr};
 
-  // ---------------- entry meeting (CTA 0, one lane per peer): x and residual_out must sit at the same offsets
+  // ---------------- entry meeting (CTA 0, one lane per peer): x and residual_out must sit at the same offsets.  It does
+  // what k::meet_peers and k::wait_grid do, written out: with those helpers ptxas schedules the reduce and norm loops
+  // differently (120 registers instead of 119) and calls of 2048-8192 rows ran 3-9% slower on an H100 (700 W).
   if (P > 1 && blockIdx.x == 0 && warp == 0) {
     bool ok = static_cast<uint32_t>(lane) == me;
     if (static_cast<uint32_t>(lane) < P && static_cast<uint32_t>(lane) != me) {
@@ -209,15 +204,11 @@ __global__ void __launch_bounds__(AR_THREADS, 1) k_plugin_ar_rmsnorm(ArRmsNormPa
       }
     }
     const uint32_t mask = __ballot_sync(0xffffffffu, ok);
-    if (lane == 0) {
-      p.flags[5] = mask;
-      __threadfence();
-      dev::st_release_gpu(&p.flags[0], 1u); // no CTA touches a peer before this release
-    }
+    if (lane == 0) k::release_grid(p.flags, mask); // no CTA touches a peer before this release
   }
   if (P > 1) {
-    wait_release(&p.flags[0], ctx);
-    if (threadIdx.x == 0) s_ok = *reinterpret_cast<volatile unsigned int *>(&p.flags[5]) | (1u << me);
+    wait_release(&p.flags[k::FLAG_RELEASE], ctx);
+    if (threadIdx.x == 0) s_ok = *reinterpret_cast<volatile unsigned int *>(&p.flags[k::FLAG_MASK]) | (1u << me);
   } else if (threadIdx.x == 0) {
     s_ok = 1u;
   }
@@ -256,9 +247,9 @@ __global__ void __launch_bounds__(AR_THREADS, 1) k_plugin_ar_rmsnorm(ArRmsNormPa
     // every CTA's pushes are performed before it arrives; CTA 0 then meets every peer once more
     __threadfence_system();
     __syncthreads();
-    if (threadIdx.x == 0) atomicAdd(&p.flags[1], 1u);
+    if (threadIdx.x == 0) atomicAdd(&p.flags[AR_PHASE1], 1u);
     if (blockIdx.x == 0 && warp == 0) {
-      if (lane == 0) k::wait_ge(&p.flags[1], G, ctx, RECEIVE_TIMEOUT_ERROR);
+      if (lane == 0) k::wait_ge(&p.flags[AR_PHASE1], G, ctx, RECEIVE_TIMEOUT_ERROR);
       __syncwarp();
       __threadfence_system();
       if (static_cast<uint32_t>(lane) < P && static_cast<uint32_t>(lane) != me) {
@@ -266,9 +257,9 @@ __global__ void __launch_bounds__(AR_THREADS, 1) k_plugin_ar_rmsnorm(ArRmsNormPa
         k::pad_wait(ctx, MAX_CH - 1, lane);
       }
       __syncwarp();
-      if (lane == 0) dev::st_release_gpu(&p.flags[2], 1u);
+      if (lane == 0) dev::st_release_gpu(&p.flags[AR_MIDDLE], 1u);
     }
-    wait_release(&p.flags[2], ctx);
+    wait_release(&p.flags[AR_MIDDLE], ctx);
     // ===== phase 2: every row of the local residual_out, written by this rank's and the peers' CTAs
     for (uint64_t row = blockIdx.x; row < p.m; row += G) {
       const char *hrow = my_heap + p.h_off + row * p.h * 2;
@@ -281,28 +272,12 @@ __global__ void __launch_bounds__(AR_THREADS, 1) k_plugin_ar_rmsnorm(ArRmsNormPa
     }
   }
 
-  // ---------------- teardown: the last CTA to finish publishes the status (one-shot: after meeting the peers again)
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    if (s_err) atomicOr(&p.flags[4], s_err);
-    __threadfence();
-    s_last = atomicAdd(&p.flags[3], 1u) == G - 1 ? 1u : 0u;
-  }
-  __syncthreads();
-  if (s_last) {
-    __threadfence();
-    // every CTA of this rank has read what it needed of the peers' x: when all ranks meet here, each may rewrite its x
-    if (P > 1 && !p.two_shot) k::chan_sync(ctx, false, 0, 0, nullptr, nullptr);
-    if (threadIdx.x == 0 && p.status) *p.status = atomicOr(&p.flags[4], s_err) | s_err;
-  }
+  // ---------------- teardown: the last CTA to finish publishes the status.  One-shot, it meets the peers first: every
+  // CTA of this rank has read what it needed of the peers' x, so when all ranks meet there, each may rewrite its x.
+  k::plugin_exit(ctx, p.flags, p.status, P > 1 && !p.two_shot, s_last);
 }
 
 // ----------------------------------------------------------------------- host
-namespace {
-std::mutex g_arn_m;
-std::map<CudaDevice *, unsigned int *> g_arn_flags;
-} // namespace
-
 void preload_ar_rmsnorm_kernels() {
   cudaFuncAttributes a;
   cudaFuncGetAttributes(&a, k_plugin_ar_rmsnorm);
@@ -326,16 +301,6 @@ cudaError_t launch_ar_rmsnorm(CudaDevice &dev, const ArRmsNormArgs &a, cudaStrea
   if (r_ptr && r_ptr != h_ptr && r_ptr < h_ptr + bytes && h_ptr < r_ptr + bytes)
     throw std::invalid_argument("ar_rmsnorm: residual overlaps residual_out without being the same tensor");
   ACCL_CUDART(cudaSetDevice(dev.device()));
-  unsigned int *flags;
-  {
-    std::lock_guard<std::mutex> lk(g_arn_m);
-    unsigned int *&f = g_arn_flags[&dev];
-    if (!f) {
-      ACCL_CUDART(cudaMalloc(&f, AR_FLAG_WORDS * sizeof(unsigned int)));
-      ACCL_CUDART(cudaMemset(f, 0, AR_FLAG_WORDS * sizeof(unsigned int)));
-    }
-    flags = f;
-  }
   ArRmsNormParams p;
   p.w = w;
   p.x_off = a.x_off;
@@ -349,14 +314,13 @@ cudaError_t launch_ar_rmsnorm(CudaDevice &dev, const ArRmsNormArgs &a, cudaStrea
   p.timeout_us = dev.timeout_us();
   // the all-reduce planner's rule (plan.hpp): one-shot while bytes x ranks fit oneshot_max_bytes
   p.two_shot = P > 1 && bytes * P > dev.config().oneshot_max_bytes ? 1u : 0u;
-  p.flags = flags;
   p.status = a.status_dev;
   int sms = 0;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev.device());
   // the kernel spins on grid-wide flags and waits for its peers: every CTA of every rank on this GPU must be resident
   const uint32_t grid = std::min<uint32_t>(std::min<uint32_t>(static_cast<uint32_t>(std::max(dev.config().max_ctas, 1)),
                                                               static_cast<uint32_t>(std::max(sms, 1))), a.m);
-  ACCL_CUDART(cudaMemsetAsync(flags, 0, AR_FLAG_WORDS * sizeof(unsigned int), stream));
+  p.flags = plugin_flags(dev, 'N', AR_FLAG_WORDS, stream);
   k_plugin_ar_rmsnorm<<<grid, AR_THREADS, 0, stream>>>(p);
   return cudaGetLastError();
 }

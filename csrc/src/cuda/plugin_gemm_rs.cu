@@ -29,6 +29,9 @@
 // Tiles are visited owner-rotated (peers' rows first, own rows last) so the
 // NVLink traffic overlaps the remaining math.  Shards are zeroed in-kernel and
 // two flag barriers over the sync pads (channel MAX_CH-1) bracket the adds.
+// The pipeline, the CTA-pair helpers and the epilogue live in wgmma.cuh; the entry meeting, the grid release and the
+// exit in kernels.cuh.  This file keeps the tile orders, the zeroing, the all-reduce signal and broadcast, and the host
+// launch code.
 //
 // GEMM -> ALL-REDUCE (AR kernels, launch_gemm_ar): the same kernel with a two-shot all-reduce epilogue.  Every rank
 // ends with the same full C [M, N] at out_off of its heap.
@@ -51,11 +54,10 @@
 
 #include <cstdlib>
 #include <cstring>
-#include <map>
-#include <mutex>
 
 #include "accl/cuda/cudadevice.hpp"
 #include "accl/cuda/driver_api.hpp"
+#include "accl/cuda/launch.hpp"
 #include "accl/cuda/plugins.hpp"
 #include "accl/device/api.cuh"
 #include "kernels.cuh"
@@ -64,52 +66,20 @@
 namespace accl {
 namespace cuda {
 
-namespace g {
-// ---- CTA-pair (cluster of 2) flavours of the primitives
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// the TMA unit writes the box at the same shared-memory offset in every CTA of `mask` and signals the barrier at
-// the same offset in each of them
-__device__ __forceinline__ void tma_load_2d_multicast(void *smem_dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1,
-                                                      uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(
-          smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
-      : "memory");
-}
-// arrive on the barrier at this shared-memory offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t *bar, uint32_t cta) {
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
-
-template <bool PAIR> struct Cfg {
-  static constexpr int BN_LOAD = PAIR ? BN / 2 : BN;          // W rows this CTA loads per stage
-  static constexpr int TILE_M = PAIR ? 2 * BM : BM;           // rows of one output tile
-};
-} // namespace g
-
 struct alignas(64) OutMaps {
   CUtensorMap m[ACCL_MAX_RANKS]; // owner rank o: its [M/P, N] shard through my peer mapping
 };
+
+// flag block (kernels.cuh, PluginFlag) of both epilogues; their own word: CTAs whose warps 1-3 have zeroed their part of C
+constexpr uint32_t GEMM_ZEROED = k::FLAG_PLUGIN, GEMM_FLAG_WORDS = GEMM_ZEROED + 1;
 
 struct GemmRsParams {
   DevWorld w;
   uint64_t out_off;
   uint32_t m, n, k;
-  uint32_t epoch;
   uint32_t timeout_us;
-  unsigned int *grid_flags; // zeroed before every launch: [0] zero-phase arrivals, [1] release, [2] finished CTAs, [3] error, [8..] peer offsets
-  uint32_t *status;         // receives the error bits (0: success) when the kernel ends; may be null
+  unsigned int *flags; // the flag block, zeroed before every launch
+  uint32_t *status;    // receives the error bits (0: success) when the kernel ends; may be null
 };
 
 struct GemmArParams : GemmRsParams {
@@ -125,24 +95,6 @@ template <> struct ParamsOf<true> { using type = GemmArParams; };
 // last block may be short; its slots past the last tile are skipped.
 __device__ __forceinline__ uint32_t ar_tile_of_slot(uint32_t s, uint32_t P, uint32_t me) { return s - s % P + (s % P + me + 1) % P; }
 
-
-template <bool F32, int C>
-__device__ __forceinline__ void emit_chunks(const float (&d)[128], uint8_t *my_epi, uint32_t &ebuf, int lane, const CUtensorMap *map,
-                                            int col0, int row) {
-  constexpr int COLS = F32 ? 32 : 64;
-  if constexpr (C < g::BN / COLS) {
-    uint8_t *buf = my_epi + ebuf * g::EPI_BUF_BYTES;
-    // the TMA unit must be done READING this buffer (issued two chunks ago)
-    if (lane == 0) device::emit_wait_read<1>();
-    __syncwarp();
-    epilogue_chunk<F32, C>(d, buf, lane);
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); // generic-proxy writes -> visible to the TMA unit
-    __syncwarp();
-    if (lane == 0) device::reduce_scatter_emit_tile(map, buf, col0 + C * COLS, row);
-    ebuf ^= 1;
-    emit_chunks<F32, C + 1>(d, my_epi, ebuf, lane, map, col0, row);
-  }
-}
 
 // GEMM -> all-reduce broadcast: one warp copies a finished TILE_M x 256 tile of its own C into the same tile of every
 // peer's C, 16 bytes per lane and access, four loads in flight.  `base`: the tile's offset from the start of a heap.
@@ -176,15 +128,7 @@ k_plugin_gemm_rs(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   using C = Cfg<PAIR>;
   constexpr int GROUP_M = PAIR ? 8 : 16;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint8_t *smem_a = smem;
-  uint8_t *smem_b = smem + STAGES * A_STAGE_BYTES;
-  uint8_t *smem_epi = smem + STAGES * STAGE_BYTES;
-  uint64_t *bars = reinterpret_cast<uint64_t *>(smem + STAGES * STAGE_BYTES + EPI_BYTES);
-  uint64_t *full = bars, *empty = bars + STAGES;
-
-  __shared__ uint32_t s_err;
-  __shared__ k::PtrTable s_tab;
+  __shared__ uint32_t s_err, s_last;
   __shared__ WorkItem s_item; // identity communicator for the sync pads
 
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
@@ -198,21 +142,10 @@ k_plugin_gemm_rs(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   char *my_heap = p.w.window + static_cast<uint64_t>(me) * p.w.heap_bytes;
 
   // ---------------- one-time setup
+  const Smem sm = gemm_smem<PAIR>(smem_raw);
   if (threadIdx.x == 0) {
     s_err = 0;
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full[i], 1);                // the producer's arrive.expect_tx
-      mbar_init(&empty[i], PAIR ? 4 : 2);    // one arrival per consumer warpgroup (pair: of both CTAs)
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    s_item.comm_size = P;
-    s_item.comm_rank = me;
-    for (uint32_t r = 0; r < static_cast<uint32_t>(ACCL_MAX_RANKS); ++r) s_item.members[r] = static_cast<uint8_t>(r < P ? r : 0);
-    s_item.desc.scenario = AR ? 0x52 : 0x47; // 'G' / 'R' (all-reduce): both ends must be in the same plugin
-    s_item.timeout_us = p.timeout_us;
-    s_item.bank = 0;
-    s_item.comm_sig = AR ? 0x474152u : 0x47454Du;
+    k::plugin_item(s_item, p.w, AR ? 0x52 : 0x47, AR ? 0x474152u : 0x47454Du, p.timeout_us); // 'R' (all-reduce) / 'G'
   }
   if (warp == 0 && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_a)) : "memory");
@@ -225,7 +158,7 @@ k_plugin_gemm_rs(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   // (warp 0) and the consumers go straight to the main loop; warps 1-3 zero the shard (the reduce-adds accumulate
   // into it), warp 3 of CTA 0 then exchanges the shard offsets with the peers on the sync pads and releases the
   // epilogues of the whole grid.  The first tile's accumulator is ready long after (K / 64 stages of MMAs).
-  k::Ctx ctx{p.w, s_item, MAX_CH - 1, 1, reinterpret_cast<Ctrl *>(my_heap), &s_err, static_cast<uint64_t>(p.timeout_us) * 1000ull, &s_tab};
+  k::Ctx ctx{p.w, s_item, MAX_CH - 1, 1, reinterpret_cast<Ctrl *>(my_heap), &s_err, static_cast<uint64_t>(p.timeout_us) * 1000ull, nullptr};
   // all-reduce: tiles owned by this rank (me, me + P, ...) and the offset of a tile's first element in C
   constexpr uint32_t ES = F32 ? 4 : 2;
   const uint32_t owned = num_tiles > me ? (num_tiles - me + P - 1) / P : 0;
@@ -253,52 +186,28 @@ k_plugin_gemm_rs(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     asm volatile("fence.proxy.async.global;" ::: "memory"); // the zeros are read by the TMA unit's reduce-adds
     __threadfence();
     asm volatile("bar.sync 1, 96;" ::: "memory"); // warps 1-3 only
-    if (threadIdx.x == 32) atomicAdd(&p.grid_flags[0], 1u);
+    if (threadIdx.x == 32) atomicAdd(&p.flags[GEMM_ZEROED], 1u);
     if (blockIdx.x == 0 && warp == 3) {
-      // the whole grid has zeroed -> meet every peer (sync pads, channel MAX_CH-1), one lane per peer
-      if (lane == 0)
-        while (atomicAdd(&p.grid_flags[0], 0u) < gridDim.x) dev::nanosleep(100);
+      // the whole grid has zeroed -> meet every peer.  The output tensor maps assume the shard (all-reduce: C and the
+      // counter block) sits at the same offset in every heap: a peer that does not answer, is in another operation or
+      // has it elsewhere gets no reduce-adds.
+      if (lane == 0) k::wait_ge(&p.flags[GEMM_ZEROED], gridDim.x, ctx, RECEIVE_TIMEOUT_ERROR);
       __syncwarp();
       __threadfence();
-      // the output tensor maps assume the shard sits at out_off in every heap: a peer that does not answer, is in
-      // another operation or has its shard elsewhere gets no reduce-adds (INVALID_OFF, or its differing offset)
-      // (all-reduce: C and the counter block both; a peer that differs in either is marked INVALID_OFF)
-      uint64_t peer_off = p.out_off, off2 = p.out_off;
+      uint64_t off2 = 0;
       if constexpr (AR) off2 = p.cnt_off;
-      if (static_cast<uint32_t>(lane) < P && static_cast<uint32_t>(lane) != me) {
-        k::pad_post(ctx, MAX_CH - 1, lane, k::REC_OFFS, p.out_off, off2, ctx.kind_word());
-        peer_off = INVALID_OFF;
-        if (k::pad_wait(ctx, MAX_CH - 1, lane)) {
-          const SyncRec r = k::pad_rec(ctx, MAX_CH - 1, lane, AR ? k::REC_OFFS : k::REC_OFF0);
-          if (r.kind != ctx.kind_word()) {
-            atomicOr(&s_err, PACK_SEQ_NUMBER_ERROR);
-          } else {
-            peer_off = r.off0;
-            if constexpr (AR)
-              if (r.off2 != off2) peer_off = INVALID_OFF;
-            if (peer_off != p.out_off) atomicOr(&s_err, DMA_MISMATCH_ERROR);
-          }
-        }
-      }
-      if (static_cast<uint32_t>(lane) < P) reinterpret_cast<volatile uint64_t *>(p.grid_flags + 8)[lane] = peer_off;
-      __threadfence();
-      __syncwarp();
-      if (lane == 0) atomicExch(&p.grid_flags[1], 1u); // release the epilogues of every CTA
+      const uint32_t mask = k::meet_peers(ctx, AR ? k::REC_OFFS : k::REC_OFF0, p.out_off, off2);
+      if (lane == 0) k::release_grid(p.flags, mask); // release the epilogues of every CTA
     }
     if constexpr (AR) {
       // ===== broadcast: this rank's owned tiles, round robin over the grid's warps 1-3, each once all P ranks' consumer
       // warps have signalled it.  Nothing is pushed unless every peer's C and counters sit where this rank's do (a
       // peer that differs gets no pushes, and the tiles it would have added are never complete).
-      if (lane == 0) {
-        uint32_t spins = 0;
-        while (*reinterpret_cast<volatile unsigned int *>(&p.grid_flags[1]) == 0)
-          if (++spins > 64) dev::nanosleep(200);
-      }
-      __syncwarp();
+      uint32_t mask = 0;
+      if (lane == 0) mask = k::wait_grid(p.flags, ctx);
+      mask = __shfl_sync(0xffffffffu, mask, 0);
       __threadfence();
-      const bool all_ok = __all_sync(0xffffffffu, static_cast<uint32_t>(lane) >= P ||
-                                                      reinterpret_cast<const volatile uint64_t *>(p.grid_flags + 8)[lane] == p.out_off);
-      if (all_ok && P > 1) {
+      if (mask == (2u << (P - 1)) - 1u && P > 1) {
         const uint32_t *cnt = reinterpret_cast<const uint32_t *>(my_heap + p.cnt_off);
         const uint32_t want = P * (C::TILE_M / EPI_ROWS); // one arrival per consumer warp of every rank
         bool waiting = true; // false after a timed-out tile: the rest are skipped
@@ -327,54 +236,18 @@ k_plugin_gemm_rs(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       uint32_t mo, nb;
       tile_coords<GROUP_M>(t, tiles_m, tiles_n, mo, nb);
       const uint32_t mb = AR ? mo : (mo + (me + 1) * tiles_m_per_rank) % tiles_m; // peers' rows first, mine last
-      for (uint32_t kb = 0; kb < k_blocks; ++kb) {
-        if (lane == 0) {
-          mbar_wait(&empty[stage], phase ^ 1); // pair: the stage is free in BOTH CTAs
-          mbar_expect_tx(&full[stage], STAGE_BYTES);
-          tma_load_2d(smem_a + stage * A_STAGE_BYTES, &tmap_a, &full[stage], static_cast<int>(kb * BK),
-                      static_cast<int>(mb * C::TILE_M + cr * BM));
-          if constexpr (KN) {
-            // W is [K, N]: this CTA's columns in boxes of 64 columns x 64 K-rows, one 8 KB column of swizzle atoms each
-#pragma unroll
-            for (int j = 0; j < C::BN_LOAD / 64; ++j) {
-              uint8_t *dst = smem_b + stage * B_STAGE_BYTES + cr * (C::BN_LOAD * BK * 2) + j * (64 * BK * 2);
-              const int n0 = static_cast<int>(nb * BN + cr * C::BN_LOAD + 64 * j), k0 = static_cast<int>(kb * BK);
-              if (PAIR)
-                tma_load_2d_multicast(dst, &tmap_b, &full[stage], n0, k0, 0x3);
-              else
-                tma_load_2d(dst, &tmap_b, &full[stage], n0, k0);
-            }
-          } else if (PAIR) {
-            tma_load_2d_multicast(smem_b + stage * B_STAGE_BYTES + cr * (C::BN_LOAD * BK * 2), &tmap_b, &full[stage],
-                                  static_cast<int>(kb * BK), static_cast<int>(nb * BN + cr * C::BN_LOAD), 0x3);
-          } else {
-            tma_load_2d(smem_b + stage * B_STAGE_BYTES, &tmap_b, &full[stage], static_cast<int>(kb * BK), static_cast<int>(nb * BN));
-          }
-        }
-        __syncwarp();
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
+      produce_tile<PAIR, KN>(sm, &tmap_a, static_cast<int>(mb * C::TILE_M + cr * BM), &tmap_b, nb, k_blocks, cr, stage, phase, lane);
     }
   } else if (warp >= 4) {
     // ===== consumers: wgmma into registers, then registers -> shard element type -> swizzled smem -> collective
     const uint32_t wg = warp / 4 - 1;   // rows [64 wg, 64 wg + 64) of the CTA's 128
     const uint32_t wi = warp % 4;       // this warp's 16 of them
-    const bool signaller = threadIdx.x % 128 == 0;
-    uint8_t *my_epi = smem_epi + (warp - 4) * 2 * EPI_BUF_BYTES;
+    uint8_t *my_epi = sm.epi + (warp - 4) * 2 * EPI_BUF_BYTES;
     uint32_t stage = 0, phase = 0, ebuf = 0;
     uint32_t owners_ok = 0; // owners whose shard sits at out_off, the only ones this warp adds into; 0: not yet released
     float d[128];
 #pragma unroll
     for (int i = 0; i < 128; ++i) d[i] = 0.f;
-    auto release = [&](uint32_t s) {
-      if (signaller) {
-        mbar_arrive(&empty[s]);
-        if (PAIR) mbar_arrive_cluster(&empty[s], cr ^ 1u); // the peer's producer multicasts into this stage too
-      }
-    };
     uint32_t pending = ~0u; // all-reduce: the tile whose adds this warp has issued but not yet signalled
     // Signal `pending`: its adds have been performed at the owner (wait_group without .read waits for the writes, not
     // only the reads of shared memory), fence.proxy.async orders those async-proxy writes before this thread's
@@ -400,41 +273,14 @@ k_plugin_gemm_rs(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       uint32_t mo, nb;
       tile_coords<GROUP_M>(t, tiles_m, tiles_n, mo, nb);
       const uint32_t mb = AR ? mo : (mo + (me + 1) * tiles_m_per_rank) % tiles_m;
-      uint32_t prev = 0;
-      for (uint32_t kb = 0; kb < k_blocks; ++kb) {
-        mbar_wait(&full[stage], phase);
-        const uint64_t da = make_smem_desc(smem_u32(smem_a + stage * A_STAGE_BYTES + wg * 64 * 128));
-        const uint32_t b_addr = smem_u32(smem_b + stage * B_STAGE_BYTES);
-        const uint64_t db = KN ? make_smem_desc_mn(b_addr) : make_smem_desc(b_addr);
-        constexpr uint64_t DB_STEP = KN ? 128 : 2; // per K=16 step, >> 4: 16 K-rows of 128 B (MN-major), 32 B (K-major)
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < BK / WGMMA_K; ++kk) // A: +32 bytes (>>4 = 2) per K=16 step inside the swizzle atom
-          wgmma_m64n256k16<KN ? 1 : 0>(d, da + 2 * kk, db + DB_STEP * kk, (kb | kk) ? 1u : 0u);
-        wgmma_commit();
-        wgmma_wait<1>(); // the previous stage's MMAs have retired: it may be refilled
-        if (kb > 0) release(prev);
-        prev = stage;
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-      wgmma_wait<0>();
-      release(prev);
+      consume_tile<PAIR, KN>(sm, d, wg, k_blocks, cr, stage, phase);
 
       if (!owners_ok) {
-        if (lane == 0) {
-          uint32_t spins = 0;
-          while (*reinterpret_cast<volatile unsigned int *>(&p.grid_flags[1]) == 0)
-            if (++spins > 64) dev::nanosleep(200);
-        }
-        __syncwarp();
+        if (lane == 0) owners_ok = k::wait_grid(p.flags, ctx);
+        owners_ok = __shfl_sync(0xffffffffu, owners_ok, 0);
         __threadfence();
         // every shard has been zeroed with generic stores: order them before this warp's TMA reduce-adds
         asm volatile("fence.proxy.async.global;" ::: "memory");
-        owners_ok = (1u << me) | __ballot_sync(0xffffffffu, static_cast<uint32_t>(lane) < P &&
-                                                              reinterpret_cast<const volatile uint64_t *>(p.grid_flags + 8)[lane] == p.out_off);
       }
       const uint32_t row0 = mb * C::TILE_M + cr * BM + wg * 64 + wi * EPI_ROWS; // first of this warp's 16 rows
       if constexpr (AR) {
@@ -442,13 +288,13 @@ k_plugin_gemm_rs(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         signal();
         const uint32_t owner = t % P;
         if ((owners_ok >> owner) & 1u) {
-          emit_chunks<F32, 0>(d, my_epi, ebuf, lane, &out_maps.m[owner], static_cast<int>(nb * BN), static_cast<int>(row0));
+          epilogue_tile<F32, true>(d, my_epi, ebuf, lane, &out_maps.m[owner], static_cast<int>(nb * BN), static_cast<int>(row0));
           pending = t;
         }
       } else {
         const uint32_t owner = row0 / rows_per_rank;                              // a warp's rows never straddle owners
         const int local_row0 = static_cast<int>(row0 - owner * rows_per_rank);
-        if ((owners_ok >> owner) & 1u) emit_chunks<F32, 0>(d, my_epi, ebuf, lane, &out_maps.m[owner], static_cast<int>(nb * BN), local_row0);
+        if ((owners_ok >> owner) & 1u) epilogue_tile<F32, true>(d, my_epi, ebuf, lane, &out_maps.m[owner], static_cast<int>(nb * BN), local_row0);
       }
     }
     signal(); // all-reduce: the last tile
@@ -457,31 +303,14 @@ k_plugin_gemm_rs(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     __threadfence_system(); // my adds are performed before this CTA reports completion
   }
 
-  // ---------------- teardown: the last CTA of the grid meets the peers again
-  __syncthreads();
+  // ---------------- teardown: the last CTA of the grid meets the peers again (every CTA of this rank has added and
+  // pushed its tiles: when all ranks meet there, every shard is complete)
   if (PAIR) cluster_sync(); // nobody exits while the peer may still signal its barriers or write its smem
-  __shared__ uint32_t s_last;
-  if (threadIdx.x == 0) {
-    if (s_err) atomicOr(&p.grid_flags[3], s_err);
-    __threadfence_system();
-    s_last = atomicAdd(&p.grid_flags[2], 1u) == gridDim.x - 1 ? 1u : 0u;
-  }
-  __syncthreads();
-  if (s_last) {
-    // every CTA of this rank has pushed its tiles: when all ranks meet here, every shard is complete
-    k::chan_sync(ctx, false, 0, 0, nullptr, nullptr);
-    if (threadIdx.x == 0 && p.status) *p.status = atomicOr(&p.grid_flags[3], s_err) | s_err;
-  }
+  k::plugin_exit(ctx, p.flags, p.status, true, s_last);
 }
 
 // ----------------------------------------------------------------------- host
 namespace {
-struct PluginState {
-  unsigned int *flags = nullptr; // 64 words
-};
-std::mutex g_state_m;
-std::map<CudaDevice *, PluginState> g_state;
-
 template <bool PAIR, bool F32, bool KN, bool AR> void set_smem_attr() {
   cudaFuncSetAttribute(k_plugin_gemm_rs<PAIR, F32, KN, AR>, cudaFuncAttributeMaxDynamicSharedMemorySize, g::SMEM_BYTES);
 }
@@ -495,16 +324,6 @@ template <bool KN, bool AR> void preload_layout() {
   set_smem_attr<false, true, KN, AR>();
   set_smem_attr<true, false, KN, AR>();
   set_smem_attr<true, true, KN, AR>();
-}
-
-PluginState *plugin_state(CudaDevice &dev) {
-  std::lock_guard<std::mutex> lk(g_state_m);
-  PluginState *st = &g_state[&dev];
-  if (!st->flags) {
-    ACCL_CUDART(cudaMalloc(&st->flags, 64 * sizeof(unsigned int)));
-    ACCL_CUDART(cudaMemset(st->flags, 0, 64 * sizeof(unsigned int)));
-  }
-  return st;
 }
 } // namespace
 
@@ -566,17 +385,17 @@ static int chosen_variant(int variant) {
   return variant ? variant : env_variant;
 }
 
-cudaError_t launch_gemm_rs(CudaDevice &dev, const GemmRsArgs &a, cudaStream_t stream) {
+// The launch of either epilogue once its arguments are checked.  Owner o's output, shard_rows x N, sits at out_off of
+// its heap (symmetric allocation; verified in-kernel: an owner whose output is elsewhere gets no adds and the call
+// reports DMA_MISMATCH_ERROR).  pair_ok: M suits the CTA-pair kernel; pair_error: what to throw when it is forced anyway.
+template <bool AR, typename Args>
+static cudaError_t launch_gemm(CudaDevice &dev, const Args &a, uint32_t shard_rows, bool pair_ok, const char *pair_error,
+                               cudaStream_t stream) {
   using namespace g;
-  const uint32_t P = dev.world().world;
-  if (a.m % (BM * P) || a.n % BN || a.k % BK)
-    throw std::invalid_argument("gemm_rs: need M % (128*world) == 0, N % 256 == 0, K % 64 == 0");
+  const DevWorld &w = dev.world();
   ACCL_CUDART(cudaSetDevice(dev.device()));
-  PluginState *st = plugin_state(dev);
-  // CTA-pair kernel: 256-row tiles must not straddle shard owners
   const int variant = chosen_variant(a.variant);
-  const bool pair_ok = a.m % (2 * BM * P) == 0;
-  if (variant == 2 && !pair_ok) throw std::invalid_argument("gemm_rs: the CTA-pair kernel needs M % (256*world) == 0");
+  if (variant == 2 && !pair_ok) throw std::invalid_argument(pair_error);
   const bool pair = variant == 2 || (variant == 0 && pair_ok);
   const bool f32 = a.out_f32;
   const CUtensorMap ta = make_map(a.a, a.m, a.k, BM, BK);
@@ -584,31 +403,40 @@ cudaError_t launch_gemm_rs(CudaDevice &dev, const GemmRsArgs &a, cudaStream_t st
   const CUtensorMap tb = a.w_kn ? make_map(a.w, a.k, a.n, BK, 64) : make_map(a.w, a.n, a.k, pair ? BN / 2 : BN, BK);
   OutMaps om;
   std::memset(&om, 0, sizeof(om));
-  for (uint32_t o = 0; o < P; ++o) // symmetric allocation: the shard sits at out_off in every heap (verified in-kernel:
-                                   // an owner whose shard is elsewhere gets no adds and the call reports DMA_MISMATCH_ERROR)
-    om.m[o] = make_map(dev.world().window + static_cast<uint64_t>(o) * dev.world().heap_bytes + a.out_off, a.m / P, a.n, EPI_ROWS,
-                       f32 ? 32 : 64, f32);
-  GemmRsParams p;
-  p.w = dev.world();
+  for (uint32_t o = 0; o < w.world; ++o)
+    om.m[o] = make_map(w.window + static_cast<uint64_t>(o) * w.heap_bytes + a.out_off, shard_rows, a.n, EPI_ROWS, f32 ? 32 : 64, f32);
+  typename ParamsOf<AR>::type p;
+  p.w = w;
   p.out_off = a.out_off;
   p.m = a.m;
   p.n = a.n;
   p.k = a.k;
-  p.epoch = a.epoch;
   p.timeout_us = dev.timeout_us();
-  p.grid_flags = st->flags;
+  p.flags = plugin_flags(dev, 'G', GEMM_FLAG_WORDS, stream);
   p.status = a.status_dev;
+  const uint32_t tiles = (a.m / (pair ? 2 * BM : BM)) * (a.n / BN);
+  if constexpr (AR) {
+    p.cnt_off = a.cnt_off;
+    // the peers add into these counters only after this launch has met them, i.e. after the memset
+    ACCL_CUDART(cudaMemsetAsync(w.window + static_cast<uint64_t>(w.rank) * w.heap_bytes + a.cnt_off, 0, tiles * sizeof(uint32_t), stream));
+  }
   int sms = 0;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev.device());
-  ACCL_CUDART(cudaMemsetAsync(st->flags, 0, 64 * sizeof(unsigned int), stream));
-  const uint32_t tiles = (a.m / (pair ? 2 * BM : BM)) * (a.n / BN);
-  return launch_kernel<false>(pair, f32, a.w_kn, ta, tb, om, p, tiles, sms, stream);
+  return launch_kernel<AR>(pair, f32, a.w_kn, ta, tb, om, p, tiles, sms, stream);
+}
+
+cudaError_t launch_gemm_rs(CudaDevice &dev, const GemmRsArgs &a, cudaStream_t stream) {
+  using namespace g;
+  const uint32_t P = dev.world().world;
+  if (a.m % (BM * P) || a.n % BN || a.k % BK)
+    throw std::invalid_argument("gemm_rs: need M % (128*world) == 0, N % 256 == 0, K % 64 == 0");
+  // CTA-pair kernel: 256-row tiles must not straddle shard owners
+  return launch_gemm<false>(dev, a, a.m / P, a.m % (2 * BM * P) == 0, "gemm_rs: the CTA-pair kernel needs M % (256*world) == 0", stream);
 }
 
 cudaError_t launch_gemm_ar(CudaDevice &dev, const GemmArArgs &a, cudaStream_t stream) {
   using namespace g;
   const DevWorld &w = dev.world();
-  const uint32_t P = w.world;
   if (!a.m || !a.n || !a.k || a.m % BM || a.n % BN || a.k % BK)
     throw std::invalid_argument("gemm_ar: need M % 128 == 0, N % 256 == 0, K % 64 == 0, none of them zero");
   if (static_cast<uint64_t>(a.m / BM) * (a.n / BN) > GEMM_AR_MAX_TILES)
@@ -616,37 +444,7 @@ cudaError_t launch_gemm_ar(CudaDevice &dev, const GemmArArgs &a, cudaStream_t st
   const uint64_t c_bytes = static_cast<uint64_t>(a.m) * a.n * (a.out_f32 ? 4 : 2);
   if (a.out_off % 16 || a.cnt_off % 16 || a.out_off + c_bytes > w.heap_bytes || a.cnt_off + GEMM_AR_MAX_TILES * 4ull > w.heap_bytes)
     throw std::invalid_argument("gemm_ar: C and the counter block must be 16-byte aligned and inside the symmetric heap");
-  ACCL_CUDART(cudaSetDevice(dev.device()));
-  PluginState *st = plugin_state(dev);
-  const int variant = chosen_variant(a.variant);
-  const bool pair_ok = a.m % (2 * BM) == 0;
-  if (variant == 2 && !pair_ok) throw std::invalid_argument("gemm_ar: the CTA-pair kernel needs M % 256 == 0");
-  const bool pair = variant == 2 || (variant == 0 && pair_ok);
-  const bool f32 = a.out_f32;
-  const CUtensorMap ta = make_map(a.a, a.m, a.k, BM, BK);
-  const CUtensorMap tb = a.w_kn ? make_map(a.w, a.k, a.n, BK, 64) : make_map(a.w, a.n, a.k, pair ? BN / 2 : BN, BK);
-  OutMaps om;
-  std::memset(&om, 0, sizeof(om));
-  for (uint32_t o = 0; o < P; ++o) // owner o's full C through my peer mapping (the offsets are verified in-kernel)
-    om.m[o] = make_map(w.window + static_cast<uint64_t>(o) * w.heap_bytes + a.out_off, a.m, a.n, EPI_ROWS, f32 ? 32 : 64, f32);
-  GemmArParams p;
-  p.w = w;
-  p.out_off = a.out_off;
-  p.m = a.m;
-  p.n = a.n;
-  p.k = a.k;
-  p.epoch = 0;
-  p.timeout_us = dev.timeout_us();
-  p.grid_flags = st->flags;
-  p.status = a.status_dev;
-  p.cnt_off = a.cnt_off;
-  int sms = 0;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev.device());
-  const uint32_t tiles = (a.m / (pair ? 2 * BM : BM)) * (a.n / BN);
-  ACCL_CUDART(cudaMemsetAsync(st->flags, 0, 64 * sizeof(unsigned int), stream));
-  // the peers add into these counters only after this launch has met them, i.e. after the memset
-  ACCL_CUDART(cudaMemsetAsync(w.window + static_cast<uint64_t>(w.rank) * w.heap_bytes + a.cnt_off, 0, tiles * sizeof(uint32_t), stream));
-  return launch_kernel<true>(pair, f32, a.w_kn, ta, tb, om, p, tiles, sms, stream);
+  return launch_gemm<true>(dev, a, a.m, a.m % (2 * BM) == 0, "gemm_ar: the CTA-pair kernel needs M % 256 == 0", stream);
 }
 
 } // namespace cuda

@@ -1,6 +1,8 @@
 // The sm_90a GEMM machinery shared by the fused GEMM plugins (plugin_gemm_rs.cu, plugin_ag_gemm.cu): tile shape and
-// shared-memory budget of the single-CTA kernel, mbarrier / TMA / wgmma / shared-memory-descriptor helpers, the L2
-// tile order and the 128B-swizzled epilogue staging, plus the host-side tensor-map encoder.
+// shared-memory budget of one CTA, mbarrier / TMA / wgmma / shared-memory-descriptor helpers and their CTA-pair
+// (cluster of 2) flavours, the shared-memory carve-up, the TMA -> mbarrier -> wgmma pipeline of one tile
+// (produce_tile / consume_tile), the L2 tile order, the 128B-swizzled epilogue (epilogue_tile), plus the host-side
+// tensor-map encoder.  Tile orders, grids and meetings stay with each plugin.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -9,6 +11,7 @@
 #include <string>
 
 #include "accl/cuda/driver_api.hpp"
+#include "accl/device/api.cuh"
 
 namespace accl {
 namespace cuda {
@@ -59,6 +62,48 @@ __device__ __forceinline__ void tma_load_2d(void *smem_dst, const CUtensorMap *m
       "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
+
+// one 16-row box of staged shared memory -> global memory by the TMA unit (a bulk group of this thread)
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap *map, const void *smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(map)),
+               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               : "memory");
+  asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+}
+
+// ---- CTA-pair (cluster of 2) flavours of the primitives
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// the TMA unit writes the box at the same shared-memory offset in every CTA of `mask` and signals the barrier at
+// the same offset in each of them
+__device__ __forceinline__ void tma_load_2d_multicast(void *smem_dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1,
+                                                      uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(
+          smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
+      : "memory");
+}
+// arrive on the barrier at this shared-memory offset in CTA `cta` of the cluster
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t *bar, uint32_t cta) {
+  uint32_t remote;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+}
+
+// PAIR: a CTA pair computes one 256 x 256 tile, each CTA 128 rows of it, and each loads half of the W tile, multicast
+// into both CTAs
+template <bool PAIR> struct Cfg {
+  static constexpr int BN_LOAD = PAIR ? BN / 2 : BN;          // W rows this CTA loads per stage
+  static constexpr int TILE_M = PAIR ? 2 * BM : BM;           // rows of one output tile
+};
 
 // K-major, 128B-swizzled shared-memory matrix descriptor (sm_90 wgmma format): rows of 128 bytes, 8-row groups
 // 1024 bytes apart; the leading byte offset is unused for swizzled K-major operands
@@ -132,6 +177,104 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t *>(&v);
 }
+
+// The dynamic shared memory of a GEMM CTA, 1024-byte aligned for the 128B swizzle: the A stages, the W stages, the
+// epilogue buffers of the consumer warps, then the full / empty barriers of the stage ring.
+struct Smem {
+  uint8_t *a, *b, *epi;
+  uint64_t *full, *empty;
+};
+
+// Carve up the dynamic shared memory; thread 0 also initialises the stage barriers.  The caller's __syncthreads (and
+// for a pair its cluster_sync) makes them visible before anything waits on or signals them.
+template <bool PAIR> __device__ __forceinline__ Smem gemm_smem(uint8_t *raw) {
+  uint8_t *base = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  uint64_t *bars = reinterpret_cast<uint64_t *>(base + STAGES * STAGE_BYTES + EPI_BYTES);
+  const Smem s{base, base + STAGES * A_STAGE_BYTES, base + STAGES * STAGE_BYTES, bars, bars + STAGES};
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&s.full[i], 1);             // the producer's arrive.expect_tx
+      mbar_init(&s.empty[i], PAIR ? 4 : 2); // one arrival per consumer warpgroup (pair: of both CTAs)
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  }
+  return s;
+}
+
+// TMA producer, lane 0 of its warp: the k-loop of one tile into the stage ring.  A: 128 rows from row_a of map_a.
+// W: this CTA's BN_LOAD rows (nk) or columns (kn, boxes of 64 columns x 64 K-rows, one 8 KB column of swizzle atoms
+// each) from column nb * BN; a pair multicasts its half into both CTAs (cr: this CTA's rank in the pair).
+template <bool PAIR, bool KN>
+__device__ __forceinline__ void produce_tile(const Smem &s, const CUtensorMap *map_a, int row_a, const CUtensorMap *map_w, uint32_t nb,
+                                             uint32_t k_blocks, uint32_t cr, uint32_t &stage, uint32_t &phase, int lane) {
+  using C = Cfg<PAIR>;
+  for (uint32_t kb = 0; kb < k_blocks; ++kb) {
+    if (lane == 0) {
+      mbar_wait(&s.empty[stage], phase ^ 1); // pair: the stage is free in BOTH CTAs
+      mbar_expect_tx(&s.full[stage], STAGE_BYTES);
+      tma_load_2d(s.a + stage * A_STAGE_BYTES, map_a, &s.full[stage], static_cast<int>(kb * BK), row_a);
+      if constexpr (KN) {
+#pragma unroll
+        for (int j = 0; j < C::BN_LOAD / 64; ++j) {
+          uint8_t *dst = s.b + stage * B_STAGE_BYTES + cr * (C::BN_LOAD * BK * 2) + j * (64 * BK * 2);
+          const int n0 = static_cast<int>(nb * BN + cr * C::BN_LOAD + 64 * j), k0 = static_cast<int>(kb * BK);
+          if (PAIR)
+            tma_load_2d_multicast(dst, map_w, &s.full[stage], n0, k0, 0x3);
+          else
+            tma_load_2d(dst, map_w, &s.full[stage], n0, k0);
+        }
+      } else if (PAIR) {
+        tma_load_2d_multicast(s.b + stage * B_STAGE_BYTES + cr * (C::BN_LOAD * BK * 2), map_w, &s.full[stage],
+                              static_cast<int>(kb * BK), static_cast<int>(nb * BN + cr * C::BN_LOAD), 0x3);
+      } else {
+        tma_load_2d(s.b + stage * B_STAGE_BYTES, map_w, &s.full[stage], static_cast<int>(kb * BK), static_cast<int>(nb * BN));
+      }
+    }
+    __syncwarp();
+    if (++stage == STAGES) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+}
+
+// Consumer warpgroup wg: the k-loop of one tile into d (rows [64 wg, 64 wg + 64) of the CTA's 128).  A stage is
+// released once its MMAs have retired, by one arrival of the warpgroup (pair: on the barriers of both CTAs, since the
+// peer's producer multicasts into it too).  Returns after every MMA of the tile has retired.
+template <bool PAIR, bool KN>
+__device__ __forceinline__ void consume_tile(const Smem &s, float (&d)[128], uint32_t wg, uint32_t k_blocks, uint32_t cr, uint32_t &stage,
+                                             uint32_t &phase) {
+  const bool signaller = threadIdx.x % 128 == 0;
+  auto release = [&](uint32_t st) {
+    if (signaller) {
+      mbar_arrive(&s.empty[st]);
+      if (PAIR) mbar_arrive_cluster(&s.empty[st], cr ^ 1u);
+    }
+  };
+  uint32_t prev = 0;
+  for (uint32_t kb = 0; kb < k_blocks; ++kb) {
+    mbar_wait(&s.full[stage], phase);
+    const uint64_t da = make_smem_desc(smem_u32(s.a + stage * A_STAGE_BYTES + wg * 64 * 128));
+    const uint32_t b_addr = smem_u32(s.b + stage * B_STAGE_BYTES);
+    const uint64_t db = KN ? make_smem_desc_mn(b_addr) : make_smem_desc(b_addr);
+    constexpr uint64_t DB_STEP = KN ? 128 : 2; // per K=16 step, >> 4: 16 K-rows of 128 B (MN-major), 32 B (K-major)
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BK / WGMMA_K; ++kk) // A: +32 bytes (>>4 = 2) per K=16 step inside the swizzle atom
+      wgmma_m64n256k16<KN ? 1 : 0>(d, da + 2 * kk, db + DB_STEP * kk, (kb | kk) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>(); // the previous stage's MMAs have retired: it may be refilled
+    if (kb > 0) release(prev);
+    prev = stage;
+    if (++stage == STAGES) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+  wgmma_wait<0>();
+  release(prev);
+}
 } // namespace g
 
 // Tile order: groups of GROUP_M tile rows are swept column by column, so the tiles in flight (one per SM) form a
@@ -172,6 +315,32 @@ __device__ __forceinline__ void epilogue_chunk(const float (&d)[128], uint8_t *b
       *reinterpret_cast<uint32_t *>(buf + r0 * 128 + off) = g::pack_bf16x2(d[4 * j], d[4 * j + 1]);
       *reinterpret_cast<uint32_t *>(buf + (r0 + 8) * 128 + off) = g::pack_bf16x2(d[4 * j + 2], d[4 * j + 3]);
     }
+  }
+}
+
+// The epilogue of one warp: its 16 accumulator rows, chunk by chunk (C of the 256 columns), through the warp's two
+// buffers `epi` (ebuf: the next one) to the TMA unit, which adds each box into the memory of `map`
+// (device API: reduce_scatter_emit_tile) with REDUCE, else stores it there.
+template <bool F32, bool REDUCE, int C = 0>
+__device__ __forceinline__ void epilogue_tile(const float (&d)[128], uint8_t *epi, uint32_t &ebuf, int lane, const CUtensorMap *map,
+                                              int col0, int row) {
+  constexpr int COLS = F32 ? 32 : 64;
+  if constexpr (C < g::BN / COLS) {
+    uint8_t *buf = epi + ebuf * g::EPI_BUF_BYTES;
+    // the TMA unit must be done READING this buffer (handed over two chunks ago)
+    if (lane == 0) device::emit_wait_read<1>();
+    __syncwarp();
+    epilogue_chunk<F32, C>(d, buf, lane);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); // generic-proxy writes -> visible to the TMA unit
+    __syncwarp();
+    if (lane == 0) {
+      if constexpr (REDUCE)
+        device::reduce_scatter_emit_tile(map, buf, col0 + C * COLS, row);
+      else
+        g::tma_store_2d(map, buf, col0 + C * COLS, row);
+    }
+    ebuf ^= 1;
+    epilogue_tile<F32, REDUCE, C + 1>(d, epi, ebuf, lane, map, col0, row);
   }
 }
 
